@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- headline benchmark of the hot path (driver contract; see DESIGN.md "Measurement").
 
-Workload (BASELINE.json metric "Poseidon perms/sec & 2^24-leaf Merkle build s at 1/2/4/8 B200"):
+Workload (BASELINE.json metric "Poseidon perms/sec & 2^24-leaf Merkle build s at 1/2/4/8 GPUs"):
 one step = one full MerkleTree::new of 2^24 two-element leaves with Poseidon CRH leaves and
 Poseidon two-to-one nodes over BN254 Fr (t=3, RF=8, RP=57, alpha=5) -- BASELINE.json configs[3].
 It fits one GPU, so the same workload runs at N = 1, 2, 4, 8 (strong scaling): the leaves are
@@ -19,6 +19,10 @@ HBM.  `e2e` = the same through the host-pointer C-ABI call (cpb_merkle_poseidon_
 pinned host memory, H2D of the leaves and D2H of both node arrays inside the timed region (a pageable
 run is reported next to it).  `configs` holds the other BASELINE configurations, each checked against
 committed oracle results.
+
+--dump-outputs DIR : after the timed steps, rank 0 writes what the last timed step returned -- the root, the top inner
+levels and a fixed, seeded sample of the leaf digests and of the inner nodes of its shard -- as DIR/<name>.npy, each
+digest as its 8 little-endian 32-bit Montgomery words in float64 (exact), so two builds can be compared output for output.
 
 --impl reference : the C restatement of the reference CPU path (oracle/cref, all usable host threads)
 on the 2^20-leaf prefix of the same leaf stream (the Rust reference cannot be built in this image).
@@ -46,9 +50,11 @@ WORKLOADS = {
     "merkle_2^20_poseidon_bls12_381": ("bls", 20, 2, BI.SEED_CONFIG2, "2^20-leaf Poseidon Merkle tree, BLS12-381 Fr default rate-2 (alpha=17, RF=8, RP=31)"),
 }
 DEFAULT_WORKLOAD = "merkle_2^24_poseidon_bn254"
-HBM_PEAK_FALLBACK = 6650.0      # GB/s, B200_PROFILING.md fallback
+HBM_PEAK_FALLBACK = 3350.0      # GB/s, NVIDIA H100 SXM data sheet (HBM3)
 CPU_LOG_SAMPLE = 20             # the CPU arm builds the tree over the first 2^20 leaves of the stream
 MASK64 = (1 << 64) - 1
+DUMP_SAMPLE = 1 << 16           # sampled leaf digests / inner nodes written by --dump-outputs (4 MB each)
+DUMP_TOP = (1 << 12) - 1        # inner nodes of the top 12 levels, heap order
 
 
 def measured_peaks():
@@ -60,6 +66,56 @@ def measured_peaks():
 
 def goldens():
     return json.load(open(os.path.join(ROOT, "tests", "golden", "bench_goldens.json")))
+
+
+def nvsmi_id(index: int) -> str:
+    """nvidia-smi's name for CUDA device `index`: its PCI bus id.  nvidia-smi numbers GPUs itself, ignoring
+    CUDA_VISIBLE_DEVICES, so a CUDA ordinal can name another physical GPU there."""
+    import torch
+    p = torch.cuda.get_device_properties(index)
+    return f"{p.pci_domain_id:08X}:{p.pci_bus_id:02X}:{p.pci_device_id:02X}.0"
+
+
+def gpu_identity(index: int):
+    """Name and power limit of the GPU a number is measured on (part of the number)."""
+    import torch
+    out = {"name": torch.cuda.get_device_name(index), "sms": torch.cuda.get_device_properties(index).multi_processor_count,
+           "pci_bus_id": nvsmi_id(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", out["pci_bus_id"], "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return out
+
+
+def digest_words_f64(t):
+    """(m, 4) int64 digest limbs (torch, any device) -> (m, 8) float64 of the little-endian 32-bit words (exact)."""
+    import numpy as np
+    return t.contiguous().cpu().numpy().view(np.uint32).reshape(-1, 8).astype(np.float64)
+
+
+def dump_outputs(out_dir, tree):
+    """The last timed step's result (this rank's view of it): root, top inner levels, seeded samples of the leaf digests
+    and inner nodes.  Indices are local to the shard; the sample depends only on the shard size."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"root": digest_words_f64(tree.root.reshape(1, 4))}
+    nodes = tree.local_nodes if tree.top_nodes is None else tree.top_nodes
+    if nodes is not None:
+        arrays["inner_nodes_top"] = digest_words_f64(nodes[:DUMP_TOP])
+    rng = np.random.default_rng(0)
+    for name, t in (("leaf_digests", tree.local_leaf_nodes), ("inner_nodes", tree.local_nodes)):
+        if t is None:
+            continue
+        m = t.shape[0]
+        idx = np.sort(rng.choice(m, size=min(m, DUMP_SAMPLE), replace=False))
+        arrays[name + "_sample"] = digest_words_f64(t[torch.from_numpy(idx).to(t.device)])
+        arrays[name + "_sample_index"] = idx.astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def u64_list(t):
@@ -79,7 +135,7 @@ class ClockSampler:
 
     def start(self):
         try:
-            self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), f"--query-gpu={self.Q}", "--format=csv,noheader,nounits",
+            self.proc = subprocess.Popen(["nvidia-smi", "-i", nvsmi_id(self.index), f"--query-gpu={self.Q}", "--format=csv,noheader,nounits",
                                           "-lms", "100"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             self.t = threading.Thread(target=self._read, daemon=True)
             self.t.start()
@@ -295,7 +351,7 @@ def run_b200(args):
             ex, use_fused = None, False
     # this rank's slice of the global leaf stream: leaves [rank*n_local, (rank+1)*n_local)
     leaves = BI.field_elements_torch(torch, N, fid, seed, rank * n_local * leaf_len, n_local * leaf_len, local_rank).view(n_local, leaf_len, 4)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)          # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)          # > 50 MB L2
     gold = goldens()
 
     def barrier():
@@ -334,6 +390,8 @@ def run_b200(args):
         root = tree.root.clone()
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, tree)
     t = torch.tensor([sum(times)], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -454,19 +512,19 @@ def run_b200(args):
     peaks = measured_peaks()
     peak = peaks["hbm_gbs"] if peaks else HBM_PEAK_FALLBACK
     achieved = alg_bytes / (k_ms * 1e-3) / 1e9
-    ncu = NCU_TRAFFIC[field_key]
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": ncu["bytes_per_hash"] * n_local, "traffic_source": ncu["source"],
                 "kernel": "k_poseidon_crh (leaf level: %d hashes of %d elements)" % (n_local, leaf_len), "kernel_ms": k_ms,
-                "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "B200_PROFILING.md fallback (of fallback)",
+                "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "H100 SXM data sheet (of fallback)",
                 "note": "the path is bound by the integer multiply pipe, not HBM (~6e4 IMAD-class instructions per 96 algorithmic bytes); see integer_pipe"}
-    sm_clock = (clocks or {}).get("sm_mhz") or 1965.0
+    gpu = gpu_identity(local_rank)
+    sm_clock = (clocks or {}).get("sm_mhz") or 1980.0   # H100 SXM maximum SM clock when the sampler has nothing
 
     def integer_pipe(fkey, prm, perms, ms, crh=False):
         w = wide_madds_per_perm(fkey, prm.rate + prm.capacity, prm.full_rounds, prm.partial_rounds, prm.alpha, crh)
-        int_peak = 148 * 32 * sm_clock * 1e6            # IMAD.WIDE: 32 lanes/clk/SM (profiles/r2_ubench_imad.txt), x sampled SM clock
+        int_peak = gpu["sms"] * 32 * sm_clock * 1e6     # IMAD.WIDE taken as half the 64/clk/SM 32-bit IMAD rate of compute capability 9.0
         return {"wide_madds_per_perm": w, "achieved_wide_madds_per_s": perms * w / (ms * 1e-3), "peak_wide_madds_per_s": int_peak,
-                "frac": perms * w / (ms * 1e-3) / int_peak, "peak_source": "148 SMs x 32 lanes/clk (measured IMAD.WIDE issue rate) x sampled SM clock"}
+                "frac": perms * w / (ms * 1e-3) / int_peak,
+                "peak_source": "%d SMs x 32 lanes/clk (assumed IMAD.WIDE issue rate, not measured) x sampled SM clock" % gpu["sms"]}
 
     integer = integer_pipe(field_key, params, n_local, k_ms, crh=True)     # the leaf kernel: one-permutation CRH
 
@@ -506,7 +564,7 @@ def run_b200(args):
                            "perms_per_step": perms_total, "inputs": "SplitMix64 stream over the global leaf index (bench_inputs.py): identical tree at every N"},
                 "root": root_u, "root_matches_oracle": root_ok, "slices_match_single_gpu_build": slices_ok,
                 "oracle_root_source": "tests/golden/bench_goldens.json (oracle/cref via tests/golden/make_bench_goldens.py)",
-                "clocks": clocks, "gpu_launches": launches_per_step * args.steps,
+                "gpu": gpu, "clocks": clocks, "gpu_launches": launches_per_step * args.steps,
                 "e2e": {"value": e2e_value, "unit": "perms/s", "h2d_bytes_per_step": n_local * leaf_len * 32 * world,
                         "d2h_bytes_per_step": (2 * n_local - 1) * 32 * world, "steps": e2e_steps, "root_matches_oracle": e2e_root_ok,
                         "api": "cpb_merkle_poseidon_build (host pointers, pinned)" if (world == 1 or ex is None) else "cpb_merkle_poseidon_build_sharded (host pointers, pinned; root exchange inside)",
@@ -519,14 +577,6 @@ def run_b200(args):
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
-
-
-# DRAM traffic of k_poseidon_crh from the committed `ncu --set full` captures (dram__bytes_read.sum + dram__bytes_write.sum of a
-# 2^20-hash, len-2 launch), per hash.  Update together with the files named here.
-NCU_TRAFFIC = {
-    "bn254": {"bytes_per_hash": (67.246848e6 + 6.766848e6) / (1 << 20), "source": "profiles/r2_ncu_crh_bn254.txt (2^20-hash launch), scaled per hash"},
-    "bls": {"bytes_per_hash": (67.188736e6 + 8.603136e6) / (1 << 20), "source": "profiles/r2_ncu_crh_bls.txt (2^20-hash launch), scaled per hash"},
-}
 
 
 def config1_probe():
@@ -558,7 +608,7 @@ def config1_probe():
 
 
 def config2(torch, cp, N, BI, gold, dev_index, flush, time_kernel, integer_pipe, hbm_peak):
-    """BASELINE configs[1]: 2^20-leaf Poseidon tree over BLS12-381 Fr on one B200, plus north_star's batched-permutation
+    """BASELINE configs[1]: 2^20-leaf Poseidon tree over BLS12-381 Fr on one GPU, plus north_star's batched-permutation
     rate (2^22 bare permutations).  Root / sampled states against the committed oracle results."""
     from crypto_primitives_b200.distributed import CudaPoseidonBackend
     prm = poseidon_params(cp, "bls")
@@ -596,7 +646,7 @@ def pedersen_setup(cp):
 
 
 def config3(torch, cp, N, BI, gold, dev_index, flush, time_kernel, integer_pipe, hbm_peak):
-    """BASELINE configs[2]: crh::pedersen + commitment::pedersen over Jubjub, window 4x256, 2^20 x 128-byte inputs, one B200."""
+    """BASELINE configs[2]: crh::pedersen + commitment::pedersen over Jubjub, window 4x256, 2^20 x 128-byte inputs, one GPU."""
     dev = torch.device("cuda", dev_index)
     prm = pedersen_setup(cp)
     t0 = time.perf_counter()
@@ -682,7 +732,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=DEFAULT_WORKLOAD, choices=list(WORKLOADS))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (root, top levels, seeded samples) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         run_reference(args)
     else:

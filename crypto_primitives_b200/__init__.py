@@ -1,10 +1,10 @@
-"""crypto_primitives_b200 -- B200-native (sm_100a CUDA) batched evaluation of the
+"""crypto_primitives_b200 -- H100-native (sm_90a CUDA) batched evaluation of the
 ark-crypto-primitives hot path: Poseidon CRH / two-to-one, Pedersen CRH / commitment, and the
 Merkle-tree build over them, behind the reference's CRHScheme / TwoToOneCRHScheme /
 CommitmentScheme / merkle_tree::Config surface.  All hashing happens in libcpb200.so
 (csrc/, C-ABI in include/cpb200.h); this package is the host-side mirror of the reference's
 interface plus ctypes plumbing.  There is no CPU fallback: importing fails without the library,
-and every compute call fails without a B200.
+and every compute call fails without an H100.
 """
 from . import _native
 from .fields import BLS12_381_FR, BLS12_377_FR, BN254_FR, JUBJUB_FR, FIELDS, Field

@@ -118,7 +118,7 @@ def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python crypto_primitives_b200/_build.py` "
-            "(nvcc, sm_100a).  crypto_primitives_b200 has no CPU fallback.")
+            "(nvcc, sm_90a).  crypto_primitives_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)       # AttributeError if the library does not export the symbol

@@ -64,6 +64,10 @@ struct DeviceGuard {
 // Number of SMs of a device (cached per device id).
 int sm_count(int device);
 
+// The library carries sm_90a code only, which loads on compute capability 9.0 (H100) and nothing else.
+bool device_is_sm90(int device);
+cpb_status check_device_arch(int device);
+
 // Stream-ordered scratch (cudaMallocAsync) is used per call; by default the driver's pool returns memory to the OS at
 // every synchronisation, which makes the next cudaMallocAsync re-map (and serialise) each time: keep it cached in the pool.
 void keep_pool_memory(int device);

@@ -1,7 +1,7 @@
 // cpb_pedersen.cu -- CUDA kernels + C-ABI for Pedersen CRH / two-to-one / commitment over a
 // twisted-Edwards curve and the Merkle builds that use them (include/cpb200.h).
 //
-// Kernels (sm_100a, integer pipe):
+// Kernels (sm_90a, integer pipe):
 //   k_pedersen_table   once per context: 256 subset sums per 8-bit chunk of the flattened generator
 //                      list, normalised to affine-Niels entries (96 B each).
 //   k_pedersen_hash    one hash per thread: for every input byte, one table lookup + one 7M mixed
@@ -219,8 +219,8 @@ k_pedersen_hash(PedersenDev P, const u32* __restrict__ consts, const u32* __rest
 
 // Wide-chunk variant: `chunk_bits` (9..16) consecutive input bits select one of 2^chunk_bits subset sums per
 // lookup, so a hash needs bits/chunk_bits mixed additions instead of bits/8.  The tables no longer fit shared
-// memory (12 bits: 33 MB for a 1024-bit input, L2-resident on a B200; 16 bits: 400 MB in HBM); each thread gathers
-// its 96-byte entry with read-only 128-bit loads.  Trades the B200's large L2/HBM for integer-pipe work.
+// memory (12 bits: 33 MB for a 1024-bit input, within the H100's 50 MB L2; 16 bits: 400 MB in HBM); each thread gathers
+// its 96-byte entry with read-only 128-bit loads.  Trades L2/HBM capacity for integer-pipe work.
 template <class F>
 __global__ void __launch_bounds__(kPedBlock)
 k_pedersen_hash_gather(PedersenDev P, const u32* __restrict__ consts, const u32* __restrict__ table,
@@ -497,7 +497,7 @@ __global__ void k_bh_children_to_bytes(const u32* __restrict__ children, uint8_t
 using namespace cpb;
 
 struct cpb_pedersen_ctx {
-    int curve_id = 0, field_id = 0, device = 0, sms = 148;
+    int curve_id = 0, field_id = 0, device = 0, sms = 132;
     int window_size = 0, num_windows = 0, n_rand = 0;
     size_t nbits = 0;
     PedersenDev dev{};
@@ -651,9 +651,8 @@ cpb_status cpb_pedersen_ctx_create_ex(int curve_id, int window_size, int num_win
     if (!out) return fail(CPB_NULL_POINTER, "null out");
     if (chunk_bits == 0) {
         // default: the widest lookup whose tables stay under 2 GiB -- 18 bits for a 1024-bit input + 252 randomness
-        // generators (1.8 GB; one gathered 96-byte entry and one mixed addition per 18 input bits; measured on a B200,
-        // 2^20 x 128-byte inputs: 8 bits 67, 12 bits 96, 16 bits 126, 18 bits 140, 20 bits 152, 22 bits 166 M hashes/s --
-        // HBM capacity traded for integer-pipe work), else 16, else 12 (L2-resident), else 8 (shared memory)
+        // generators (1.8 GB; one gathered 96-byte entry and one mixed addition per 18 input bits: HBM capacity traded for
+        // integer-pipe work), else 16, else 12 (L2-resident), else 8 (shared memory)
         const size_t bits_total = (size_t)window_size * num_windows + n_rand;
         chunk_bits = kDefaultChunkBits;
         for (int cand : {18, 16, 12}) {
@@ -688,9 +687,7 @@ cpb_status cpb_pedersen_ctx_create_ex(int curve_id, int window_size, int num_win
 
     DeviceGuard g(device);
     if (!g.ok) { cudaGetLastError(); return fail(CPB_NO_DEVICE, "cudaSetDevice(%d) failed: no usable CUDA device", device); }
-    int major = 0;
-    CPB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 10) return fail(CPB_NO_DEVICE, "device %d is sm_%d0; this library is built for sm_100a only", device, major);
+    CPB_TRY(check_device_arch(device));
 
     keep_pool_memory(device);
     cpb_pedersen_ctx* c = new cpb_pedersen_ctx();
@@ -966,7 +963,7 @@ cpb_status cpb_merkle_mixed_build(cpb_pedersen_ctx* leaf, cpb_poseidon_ctx* node
 
 // ======================================================================= Bowe-Hopwood C ABI
 struct cpb_bowe_hopwood_ctx {
-    int curve_id = 0, field_id = 0, device = 0, sms = 148;
+    int curve_id = 0, field_id = 0, device = 0, sms = 132;
     int window_size = 0, num_windows = 0, m = 4;
     size_t n_gens = 0;
     u32* d_consts = nullptr;
@@ -1053,9 +1050,7 @@ cpb_status cpb_bowe_hopwood_ctx_create(int curve_id, int window_size, int num_wi
     }
     DeviceGuard g(device);
     if (!g.ok) { cudaGetLastError(); return fail(CPB_NO_DEVICE, "cudaSetDevice(%d) failed: no usable CUDA device", device); }
-    int major = 0;
-    CPB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 10) return fail(CPB_NO_DEVICE, "device %d is sm_%d0; this library is built for sm_100a only", device, major);
+    CPB_TRY(check_device_arch(device));
 
     keep_pool_memory(device);
     cpb_bowe_hopwood_ctx* c = new cpb_bowe_hopwood_ctx();

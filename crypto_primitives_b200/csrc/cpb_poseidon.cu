@@ -1,7 +1,7 @@
 // cpb_poseidon.cu -- CUDA kernels + C-ABI for the Poseidon part of the hot path and the
 // field-leaf Merkle build on top of it (include/cpb200.h).
 //
-// Kernels (sm_100a, integer pipe, no tensor cores):
+// Kernels (sm_90a, integer pipe, no tensor cores):
 //   k_poseidon_crh      one CRH::evaluate per thread (R/crh/poseidon/mod.rs:30-40); with len==2
 //                       it is also TwoToOneCRH::compress (:66-79) and one Merkle level
 //                       (R/merkle_tree/mod.rs:454-515), because a level's children are contiguous
@@ -43,13 +43,29 @@ int sm_count(int device) {
     static int cache[64];
     static std::mutex mu;
     std::lock_guard<std::mutex> g(mu);
-    if (device < 0 || device >= 64) return 148;
+    if (device < 0 || device >= 64) return 132;
     if (!cache[device]) {
         int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || v <= 0) v = 132;
         cache[device] = v;
     }
     return cache[device];
+}
+bool device_is_sm90(int device) {
+    int major = 0, minor = 0;
+    if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device) != cudaSuccess ||
+        cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return major == 9 && minor == 0;
+}
+cpb_status check_device_arch(int device) {
+    if (device_is_sm90(device)) return CPB_OK;
+    int major = 0, minor = 0;             // only to name the device in the error
+    CPB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
+    CPB_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+    return fail(CPB_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
 }
 
 template <class F>
@@ -125,8 +141,8 @@ PoseidonDev to_dev(const host::PoseidonSchedule& S) {
         case CPB_BLS12_377_FR: CPB_FOR_T(Bls12_377_Fr, M, __VA_ARGS__)               \
     }
 
-// Largest level (in hashes) handled by the four-warp tree-top kernel: beyond ~6000 hashes the GPU's 592 warp
-// schedulers are all busy with one hash per thread anyway, and the kernel's grid is capped at 128 CTAs of 32 hashes.
+// Largest level (in hashes) handled by the four-warp tree-top kernel: beyond ~6000 hashes the GPU's 528 warp
+// schedulers (132 SMs) are all busy with one hash per thread anyway, and the kernel's grid is capped at 128 CTAs of 32 hashes.
 // CPB_TEAM_MAX overrides (0 disables; values above 4096 are clamped).
 size_t team_max() {
     static long v = -1;
@@ -140,8 +156,7 @@ size_t team_max() {
 }
 // Hand-over point of a subtree to the tree-top kernel when S subtrees are built concurrently: the four-warp kernel spends
 // ~1.4x the multiplications of the one-hash-per-thread kernel to halve the dependent chain, which pays only once the GPU is
-// latency-bound -- about 8192 hashes in flight over all streams (measured, profiles/r2_exp_team_max.txt: 2^21-leaf BN254
-// tree, overhead over the bulk rate 2.9 / 2.3 / 1.9 / 2.0 ms for per-subtree limits 4096 / 2048 / 1024 / 256 at S = 8).
+// latency-bound -- about 8192 hashes in flight over all streams (sweep the per-subtree limit with tools/perf_merkle_sizes.py).
 // CPB_TEAM_MAX, when set, is the per-subtree limit as given.
 size_t team_max_for(size_t S) {
     if (getenv("CPB_TEAM_MAX")) return team_max();
@@ -368,10 +383,8 @@ int cpb_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
     int ok = 0;
-    for (int d = 0; d < n; d++) {
-        int major = 0;
-        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, d) == cudaSuccess && major == 10) ok++;
-    }
+    for (int d = 0; d < n; d++)
+        if (device_is_sm90(d)) ok++;
     return ok;
 }
 
@@ -536,9 +549,7 @@ cpb_status cpb_poseidon_ctx_create(int field_id, int rate, int capacity, int ful
 
     DeviceGuard g(device);
     if (!g.ok) { cudaGetLastError(); return fail(CPB_NO_DEVICE, "cudaSetDevice(%d) failed: no usable CUDA device", device); }
-    int major = 0;
-    CPB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 10) return fail(CPB_NO_DEVICE, "device %d is sm_%d0; this library is built for sm_100a only", device, major);
+    CPB_TRY(check_device_arch(device));
 
     keep_pool_memory(device);          // the tree-top launches take their progress words from the stream-ordered pool
     cpb_poseidon_ctx* c = new cpb_poseidon_ctx();

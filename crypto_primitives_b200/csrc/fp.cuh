@@ -176,8 +176,8 @@ template <class F> CPB_HD void fp_double(u32* r, const u32* a) { fp_add<F>(r, a,
 namespace detail {
 
 // V += m*p with m chosen so the low limb of V = E + 2^32*O becomes zero.
-// On the B200 a 32x32->64 multiply-add (IMAD.WIDE / IMAD.HI) occupies the fmaheavy pipe twice as
-// long as a 32-bit IMAD or an ALU op, and the ALU pipe is mostly idle in this code, so moduli with
+// A 32x32->64 multiply-add (IMAD.WIDE / IMAD.HI) occupies the integer multiply pipe longer than a
+// 32-bit IMAD or an ALU op, and the ALU pipe is mostly idle in this code, so moduli with
 // trivial low limbs trade multiplies for adds:
 //   p[0] == 1          : m = -E[0];  E[0] + m*1 is exactly 2^32 when E[0] != 0, i.e. just a carry.
 //   p[1] == 2^32 - 1   : m*(2^32-1) = (m - [m!=0]) * 2^32 + E[0]   (two adds, no multiply).

@@ -1,4 +1,4 @@
-// ptx.cuh -- carry-chain integer primitives for 256-bit modular arithmetic on sm_100a.
+// ptx.cuh -- carry-chain integer primitives for 256-bit modular arithmetic on sm_90a.
 //
 // On the device every primitive is exactly one PTX instruction; ptxas fuses each
 // mad.lo.cc/madc.hi.cc pair into one IMAD.WIDE.U32(.X) with predicate carry (checked with

@@ -1,5 +1,5 @@
 /*
- * cpb200.h -- C ABI of libcpb200.so: B200-native (sm_100a) batched evaluation of the
+ * cpb200.h -- C ABI of libcpb200.so: H100-native (sm_90a) batched evaluation of the
  * ark-crypto-primitives hot path (Poseidon CRH / two-to-one, Pedersen CRH / commitment,
  * Merkle-tree build).  This is the drop-in boundary: plain pointers and sizes, no C++ or
  * torch types.  A Rust shim crate binds these symbols and implements the reference traits on
@@ -26,7 +26,7 @@
  * shim maps codes back to the reference's behaviour (R/lib.rs:46-52 `Error`, and the panics at
  * R/crh/pedersen/mod.rs:82-89, R/merkle_tree/mod.rs:430-433).  cpb_last_error() returns a
  * thread-local description of the last failure.  There is NO CPU fallback: without a usable
- * sm_100 device every compute entry point fails with CPB_NO_DEVICE / CPB_CUDA_ERROR.
+ * sm_90 (H100) device every compute entry point fails with CPB_NO_DEVICE / CPB_CUDA_ERROR.
  *
  * THREADING.  A context is immutable after creation and may be used from several host
  * threads concurrently (reference: `Parameters: Sync`, R/crh/mod.rs:21); host-pointer calls

@@ -1,4 +1,4 @@
-//! `cpb200` -- ark-crypto-primitives traits over the B200 library (`include/cpb200.h`).
+//! `cpb200` -- ark-crypto-primitives traits over the H100 library (`include/cpb200.h`).
 //!
 //! SOURCE ONLY (not compiled in this repository: the image has no Rust toolchain).  It shows exactly what a
 //! maintainer binds: the raw `extern "C"` block mirrors `include/cpb200.h`; the wrappers implement

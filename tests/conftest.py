@@ -23,15 +23,15 @@ _ensure_library()
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a device)")
 
 
 def pytest_collection_modifyitems(config, items):
-    """`pytest tests` on a machine without a B200 skips the gpu-marked tests instead of failing with CPB_NO_DEVICE."""
+    """`pytest tests` on a machine without an H100 skips the gpu-marked tests instead of failing with CPB_NO_DEVICE."""
     from crypto_primitives_b200 import _native as N
     if N.lib.cpb_device_count() > 0:
         return
-    skip = pytest.mark.skip(reason="no sm_100 device visible (cpb_device_count() == 0)")
+    skip = pytest.mark.skip(reason="no sm_90 device visible (cpb_device_count() == 0)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

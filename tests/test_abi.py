@@ -71,7 +71,7 @@ def test_ctx_create_validates_before_touching_the_gpu():
     assert N.lib.cpb_poseidon_ctx_create(0, 2, 1, 8, 31, 17, bad.ctypes.data_as(N.u64p), m.ctypes.data_as(N.u64p), 0, C.byref(out)) == N.CPB_BAD_PARAMS
 
 
-@pytest.mark.skipif(N.lib.cpb_device_count() > 0, reason="a B200 is present")
+@pytest.mark.skipif(N.lib.cpb_device_count() > 0, reason="an H100 is present")
 def test_no_cpu_fallback_without_device():
     """Without a GPU the compute path must fail loudly, never fall back."""
     cfg = cp.get_default_poseidon_parameters(cp.BLS12_381_FR, 2, False)

@@ -1,13 +1,12 @@
 // fp52.cuh -- EXPERIMENT, not part of the library: 256-bit Montgomery arithmetic on the FP64 pipe (5 limbs of 52 bits,
-// radix R' = 2^260).  Outcome on a B200 (tools/ubench_modmul.cu, profiles/r1_ubench_modmul.txt): bit-exact, but 0.90x
-// (BLS12-381 Fr) / 0.94x (BN254 Fr) the throughput of the IMAD.WIDE path of csrc/fp.cuh.  A DFMA takes two issue
+// radix R' = 2^260).  Bit-exact; tools/ubench_modmul.cu times it against the IMAD.WIDE path of csrc/fp.cuh.  A DFMA takes two issue
 // cycles and a 52x52-bit product needs three FP64 instructions plus four integer ones (two 64-bit adds): 2704 bit-products
 // per ~10 issue cycles against 1024 per 4 for IMAD.WIDE -- the same multiplier throughput per issue slot, and the SM
-// issues one instruction per cycle per scheduler whichever pipe it goes to.  Kept because the negative result is
-// measured, not assumed, and because the emulation / range-assertion scaffolding is reusable.
+// issues one instruction per cycle per scheduler whichever pipe it goes to.  Kept because the emulation / range-assertion
+// scaffolding is reusable.
 //
-// Idea: on a B200 a 32x32->64 multiply-add (IMAD.WIDE) issues at 32 lanes/clk/SM, a double-precision FMA at 64, and a
-// DFMA delivers a 52x52-bit product half where the IMAD delivers 32x32 (tools/ubench_fp64.cu, profiles/r1_ubench_fp64.txt):
+// Idea: a 32x32->64 multiply-add (IMAD.WIDE) issues at 32 lanes/clk/SM, a double-precision FMA at 64, and a
+// DFMA delivers a 52x52-bit product half where the IMAD delivers 32x32 (tools/ubench_fp64.cu):
 // about 2.5x the multiplier throughput for big-integer work, on a pipe fp.cuh leaves idle.
 //
 // How (the double-precision technique of Emmart, Zheng & Weems): for integers a, b < 2^52 held exactly in doubles,

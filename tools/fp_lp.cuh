@@ -1,12 +1,11 @@
-// fp_lp.cuh -- PROTOTYPE (measured, not used by the library): LIMB-PARALLEL 256-bit Montgomery arithmetic, one field element
+// fp_lp.cuh -- PROTOTYPE (not used by the library): LIMB-PARALLEL 256-bit Montgomery arithmetic, one field element
 // per 8 lanes of a warp, lane g holds limb g -- the "one warp per permutation, warp-shuffle" mapping BASELINE.json's
-// north_star sketches.  tools/ubench_lp.cu checks it bit for bit against csrc/fp.cuh and times it: on a B200 a dependent
-// multiplication costs 1401 cycles this way against 736-875 cycles with one thread per element (profiles/r2_ubench_lp.txt):
-// about 25 dependent shuffle / ballot steps of ~25-30 cycles each replace the multiplier-pipe time they save.  Kept as the
-// record of that experiment.
+// north_star sketches.  tools/ubench_lp.cu checks it bit for bit against csrc/fp.cuh and times it: about 25
+// dependent shuffle / ballot steps per multiplication replace the multiplier-pipe time they save.  Kept as the record of
+// that experiment.
 //
-// Idea: the small levels of a Merkle tree are bound by the dependent chain of multiplications, and a lone warp needs ~860
-// cycles for one fp_mul (136 IMAD.WIDE at 4 issue cycles each on ONE scheduler, fp.cuh).  Spreading the 64 limb products of
+// Idea: the small levels of a Merkle tree are bound by the dependent chain of multiplications, and a lone warp needs
+// one fp_mul (136 IMAD.WIDE at 4 issue cycles each on ONE scheduler, fp.cuh).  Spreading the 64 limb products of
 // a multiplication over 8 lanes makes the chain short instead: every lane does 8 wide multiply-adds per 256x256 product,
 // and carries are resolved across lanes a few times per multiplication instead of once per instruction.
 //

@@ -27,4 +27,4 @@ for rate in range(2, 9):
     dot = lambda k: 8 * (6 * k + 6)          # BLS12-381: 6 wides per row per term + 6 per reduction row
     wides = rf * (t * sbox + t * dot(t)) + rp * (sbox + dot(t) + (t - 1) * 112)
     print(f"t={t} (rate {rate}, {rf}+{rp} rounds, sparse={cp._native.lib.cpb_poseidon_ctx_is_sparse(ctx)}): {ms:.3f} ms  {n / ms / 1e3:.2f} M perms/s"
-          f"  ~{wides / 1e3:.1f}k wide madds/perm -> {n * wides / (ms * 1e-3) / (148 * 32 * 1.965e9):.2f} of the issue peak", flush=True)
+          f"  ~{wides / 1e3:.1f}k wide madds/perm -> {n * wides / (ms * 1e-3) / (132 * 32 * 1.98e9):.2f} of the issue peak", flush=True)

@@ -1,8 +1,8 @@
-// ubench_fp64.cu -- is the FP64 pipe of a B200 a second multiplier for big-integer arithmetic?
+// ubench_fp64.cu -- is the FP64 pipe of an H100 a second multiplier for big-integer arithmetic?
 // Measures DFMA / DADD / 64-bit integer add issue rates and whether DFMA overlaps with IMAD.WIDE and with ALU work.
 // (Background: 52-bit-limb Montgomery multiplication on the FP64 pipe -- two round-toward-zero FMAs give the high and
 // low halves of a 104-bit product, column sums are 64-bit integer adds on the raw bit patterns.)
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_fp64 ubench_fp64.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_fp64 ubench_fp64.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

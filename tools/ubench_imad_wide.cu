@@ -1,9 +1,9 @@
 // ubench_imad_wide.cu -- the denominator of the integer roofline: how many IMAD.WIDE.U32 (32x32+64 -> 64 multiply-add)
-// thread-operations per clock does one SM of a B200 issue?  NACC independent 64-bit accumulators per thread (no dependent
+// thread-operations per clock does one SM of an H100 issue?  NACC independent 64-bit accumulators per thread (no dependent
 // chain shorter than NACC instructions), nothing else in the loop (cuobjdump -sass: the body is NACC x UNROLL IMAD.WIDE.U32
 // plus the loop counter), long enough that launch overhead is < 0.1 %.  Also the carry-chained form the field code uses
 // (IMAD.WIDE.U32.X with predicate carry-in / carry-out).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_imad_wide ubench_imad_wide.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_imad_wide ubench_imad_wide.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
-// ubench_int.cu -- integer-pipe microbenchmark for sm_100a: how many IMAD / IMAD.WIDE /
-// IADD3 warp-instructions per clock per SM does a B200 sustain?  These are the denominators of
+// ubench_int.cu -- integer-pipe microbenchmark for sm_90a: how many IMAD / IMAD.WIDE /
+// IADD3 warp-instructions per clock per SM does an H100 sustain?  These are the denominators of
 // the integer roofline in DESIGN.md (the Poseidon/Pedersen kernels are IMAD-bound, not HBM-bound).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_int ubench_int.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_int ubench_int.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

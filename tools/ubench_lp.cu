@@ -2,9 +2,7 @@
 // arithmetic: (1) bit-exactness of lp_mul / lp_add / lp_sub against fp_mul / fp_add / fp_sub on pattern-limb operands (limbs
 // drawn from {0, 1, 2^32-1, 2^31, 2^32-2, random}: every carry path is hit constantly), (2) latency of a dependent chain of
 // multiplications for a lone warp -- what bounds the small levels of a tree.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -I crypto_primitives_b200/csrc -o tools/ubench_lp tools/ubench_lp.cu
-// Result on a B200 (profiles/r2_ubench_lp.txt): bit-exact on 2.6 M pattern-limb operand pairs over four fields; a dependent
-// multiplication costs 1401 cycles limb-parallel against 736-875 with one thread per element -- the prototype is NOT used.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I crypto_primitives_b200/csrc -o tools/ubench_lp tools/ubench_lp.cu
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>

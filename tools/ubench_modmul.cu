@@ -1,7 +1,7 @@
-// ubench_modmul.cu -- 256-bit Montgomery multiplication throughput on a B200: the IMAD.WIDE path of csrc/fp.cuh against
+// ubench_modmul.cu -- 256-bit Montgomery multiplication throughput on an H100: the IMAD.WIDE path of csrc/fp.cuh against
 // the FP64-pipe path of tools/fp52.cuh, same dependent chain per thread (x <- x*y, x <- x^2 alternating), and a
 // bit-for-bit check of the GPU results against the host build of the very same functions (exact emulation).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xptxas -v -o ubench_modmul ubench_modmul.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xptxas -v -o ubench_modmul ubench_modmul.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
