@@ -427,28 +427,31 @@ template <class F, int T> CPB_HD constexpr bool dot_needs_x() {
 }
 // The reduced value is (sum_j a_j*b_j + M*p) / R with M < R and a_j, b_j < p, i.e. below p * (T*p/R + 1): the number of
 // conditional subtractions reduce9 needs is the smallest K with T*p <= (2^(K+1) - 1) * R (again on the top limb).  One pass
-// for BN254 Fr up to T = 5 (three-term rows: 1.57 p), two for BLS12-381 Fr at T = 3 (2.36 p).
-template <class F, int T> CPB_HD constexpr int dot_reduce_passes() {
+// for BN254 Fr up to T = 5 (three-term rows: 1.57 p), two for BLS12-381 Fr at T = 3 (2.36 p).  U > 0: a term below U*p is added
+// to the reduced value (fp_dot_unit), i.e. the smallest K with T*p <= (2^(K+1) - 1 - U) * R.
+template <class F, int T, int U = 0> CPB_HD constexpr int dot_reduce_passes() {
     int k = 0;
-    while ((u64)T * ((u64)F::P(7) + 1) > (((u64)2 << k) - 1) * ((u64)1 << LIMB_BITS)) k++;
+    while ((long long)T * ((long long)F::P(7) + 1) > (((long long)2 << k) - 1 - U) * ((long long)1 << LIMB_BITS)) k++;
     return k;
 }
 
-template <class F, int T, int I, int EX> CPB_HD void dot_row(u32* E, u32* O, u32& X, const u32 (&a)[T][8], const u32* b, const u32* pm) {
-    constexpr bool WX = dot_needs_x<F, T + EX>();
-    // b: T constants of 8 limbs each (shared memory); this row uses limb I of each
+// One CIOS row over the terms J0 .. T-1 of a (b holds their T - J0 constants).
+template <class F, int T, int I, int EX, int J0 = 0>
+CPB_HD void dot_row(u32* E, u32* O, u32& X, const u32 (&a)[T][8], const u32* b, const u32* pm) {
+    constexpr bool WX = dot_needs_x<F, T - J0 + EX>();
+    // b: T - J0 constants of 8 limbs each (shared memory); this row uses limb I of each
     if (I == 0) {
         u32 bi = b[0];
 #pragma unroll
         for (int j = 0; j < 8; j += 2) {
-            mul_wide(E[j], E[j + 1], a[0][j], bi);
-            mul_wide(O[j], O[j + 1], a[0][j + 1], bi);
+            mul_wide(E[j], E[j + 1], a[J0][j], bi);
+            mul_wide(O[j], O[j + 1], a[J0][j + 1], bi);
         }
     } else {
-        shift_acc_row_x<WX>(E, O, X, a[0], b[I]);
+        shift_acc_row_x<WX>(E, O, X, a[J0], b[I]);
     }
 #pragma unroll
-    for (int t = 1; t < T; t++) acc_row_x<WX>(E, O, X, a[t], b[8 * t + I]);
+    for (int t = J0 + 1; t < T; t++) acc_row_x<WX>(E, O, X, a[t], b[8 * (t - J0) + I]);
     if (WX) redc_row_x<F>(E, O, X, pm);
     else redc_row<F>(E, O, pm);
 }
@@ -476,6 +479,37 @@ template <class F, int T, int EX = 0> CPB_HD void fp_dot(u32* r, const u32 (&a)[
     w[8] = addc(X, 0);
     // value < p * (T*p/R + 1) <= 2^(K+1) * p
     constexpr int K = detail::dot_reduce_passes<F, T + EX>();
+    detail::reduce9<F, K>(w);
+#pragma unroll
+    for (int i = 0; i < 8; i++) r[i] = w[i];
+}
+
+// r = a[0] + sum_{1<=j<T} a[j] * b[j-1] / R mod p, fully reduced: a row whose coefficient of a[0] is one (R in Montgomery form),
+// as the sparse partial rounds with a scaled lane 0 have (poseidon_host.hpp).  The unit term costs additions, not a product:
+// a[0]*R/R is added to the reduced (T-1)-term sum before the final conditional subtractions, value < XI*p + p*((T-1)*p/R + 1).
+// a[1..T-1], b[j] in [0,p); a[0] < XI * p (XI = 2: an output of the LAZY multiplier).  r must not alias a.
+template <class F, int T, int XI> CPB_HD void fp_dot_unit(u32* r, const u32 (&a)[T][8], const u32* b, const u32* pm) {
+    static_assert(T >= 2, "fp_dot_unit needs at least one product term");
+    u32 ev[8], od[8], X = 0;
+    detail::dot_row<F, T, 0, 0, 1>(ev, od, X, a, b, pm);
+    detail::dot_row<F, T, 1, 0, 1>(od, ev, X, a, b, pm);
+    detail::dot_row<F, T, 2, 0, 1>(ev, od, X, a, b, pm);
+    detail::dot_row<F, T, 3, 0, 1>(od, ev, X, a, b, pm);
+    detail::dot_row<F, T, 4, 0, 1>(ev, od, X, a, b, pm);
+    detail::dot_row<F, T, 5, 0, 1>(od, ev, X, a, b, pm);
+    detail::dot_row<F, T, 6, 0, 1>(ev, od, X, a, b, pm);
+    detail::dot_row<F, T, 7, 0, 1>(od, ev, X, a, b, pm);
+    u32 w[9];
+    w[0] = add_cc(ev[0], od[1]);
+#pragma unroll
+    for (int i = 1; i < 7; i++) w[i] = addc_cc(ev[i], od[i + 1]);
+    w[7] = addc_cc(ev[7], 0);
+    w[8] = addc(X, 0);
+    w[0] = add_cc(w[0], a[0][0]);
+#pragma unroll
+    for (int i = 1; i < 8; i++) w[i] = addc_cc(w[i], a[0][i]);
+    w[8] = addc(w[8], 0);
+    constexpr int K = detail::dot_reduce_passes<F, T - 1, XI>();
     detail::reduce9<F, K>(w);
 #pragma unroll
     for (int i = 0; i < 8; i++) r[i] = w[i];

@@ -32,6 +32,13 @@ template <class F, int T> CPB_HD void pos_add_vec(u32 (&s)[T][8], const u32* c) 
     }
 }
 
+// Offset of the matrix of full round fr (0 .. rf-1): Mpre for the last first-half round, Mpost (stored right after Mpre) for the
+// first second-half round, M otherwise.  Dense schedules store M in both slots.
+CPB_HD int pos_full_matrix(const PoseidonDev& P, int fr) {
+    const int half = P.rf / 2;
+    return fr == half - 1 ? P.off_mpre : fr == half ? P.off_mpre + P.t * P.t : P.off_m;
+}
+
 // (s0, s1, ..., s_{T-1}) <- (s1, ..., s_{T-1}, s0).  Lets a rolled loop visit every lane while
 // the state stays in registers (register files cannot be indexed dynamically); a rotation is
 // 8T moves against ~900 instructions of work per visit.
@@ -126,7 +133,7 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
                 else pos_sbox<F>(s[0], P.alpha, top_bit, pm, lazy);
                 pos_rotl<T>(s);
             }
-            const u32* rows = cs + 8 * ((phase == 0 && q == half - 1) ? P.off_mpre : P.off_m);
+            const u32* rows = cs + 8 * pos_full_matrix(P, phase * half + q);
 #pragma unroll 1
             for (int i = 0; i < T; i++) {
                 u32 d[8];
@@ -143,13 +150,15 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
             pos_add_vec<F, T>(s, cs + 8 * P.off_cp0);
             const u32* row = cs + 8 * P.off_sp;
             const u32* pc = cs + 8 * (P.off_pc + 1);
-            // Partial rounds, lazy lane 0: lane 0 lives in [0, 2p) from the constant
+            // Lane 0 is carried scaled (poseidon_host.hpp), so the row's coefficient of the S-box output y is one: the row is
+            // y + sum_{j>=1} w_j * s_j (fp_dot_unit), T-1 products instead of T.
+            // Lazy lane 0 (LZ): lane 0 lives in [0, 2p) from the constant
             // addition to the end of the round.  With a, b < 2p the Montgomery product (a*b + M*p)/R is below p*(4p/R + 1) <= 2p,
-            // so x^2, x^4, x^5 need no conditional subtraction, nor does x = d + c (d, c < p).  Consumers: the row product
-            // takes sum_j a_j < (T+1)*p (EX = 1: same code as T canonical terms when (T+2)*p <= 2^256, which is the
-            // condition below) and returns a canonical d; the column products v_j * y are ordinary multiplications whose full
-            // operand y + p stays below 2^256 and whose results are reduced, so lanes 1.. stay canonical.  Saves 4 conditional
-            // subtractions (68 instructions) per partial round; bit-identical outputs.
+            // so x^2, x^4, x^5 need no conditional subtraction, nor does x = d + c (d, c < p).  Consumers: the row adds y < 2p
+            // to the (T-1)-term sum over canonical lanes, value < 2p + p*((T-1)*p/R + 1) < 4p, and returns a canonical d; the
+            // column products v_j * y are ordinary multiplications whose full operand y + p stays below 2^256 and whose results
+            // are reduced, so lanes 1.. stay canonical.  Saves 4 conditional subtractions (68 instructions) per partial round;
+            // bit-identical outputs.
 #pragma unroll 1
             for (int k = 0; k < P.rp; k++, row += 8 * (2 * T - 1), pc += 8) {
 #if CPB_SBOX5
@@ -163,7 +172,7 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
                 if (alpha_zero) fp_one<F>(s[0]);
                 else pos_sbox<F>(s[0], P.alpha, top_bit, pm);
                 u32 d[8];
-                fp_dot<F, T, LZ ? 1 : 0>(d, s, row, pm);
+                fp_dot_unit<F, T, LZ ? 2 : 1>(d, s, row + 8, pm);       // row = [one, w_hat[1..T-1]]
                 const u32* v = row + 8 * T;
                 if (T <= CPB_COL_UNROLL_MAX) {
 #pragma unroll
@@ -240,7 +249,7 @@ template <class F, int T> CPB_HD void pos_permute(u32 (&s)[T][8], const Poseidon
         }
         // --- linear layer
         const bool dense = full || !P.sparse;
-        const u32* rows = dense ? cs + 8 * ((full && r == half - 1) ? P.off_mpre : P.off_m)
+        const u32* rows = dense ? cs + 8 * (full ? pos_full_matrix(P, r < half ? r : r - P.rp) : P.off_m)
                                 : cs + 8 * (P.off_sp + k * (2 * T - 1));
         const int nrows = dense ? T : 1;
         u32 d[8];

@@ -125,10 +125,11 @@ struct PoseidonSchedule {
     u64 alpha = 0;
     int off_c = 0;     // rf x t   constants added before the s-box of full round fr (0..rf-1)
     int off_m = 0;     // t x t    MDS
-    int off_mpre = 0;  // t x t    matrix of the last first-half full round (= D0*M; M when dense)
+    int off_mpre = 0;  // 2 x t x t: Mpre, the matrix of the last first-half full round (= D0*M; M when dense), then
+                       //          Mpost, that of the first second-half full round (M with column 0 scaled; M when dense)
     int off_cp0 = 0;   // t        constant vector added before the first partial round
     int off_pc = 0;    // rp       lane-0 constant added after partial round k-1 (entry k; entry 0 unused)
-    int off_sp = 0;    // rp x (2t-1): per round the row [m00, w_hat[1..t-1]] then v[1..t-1]  (sparse)
+    int off_sp = 0;    // rp x (2t-1): per round the row [one, w_hat[1..t-1]] then v[1..t-1]  (sparse; lane 0 scaled)
     int off_arkp = 0;  // rp x t   original partial-round constants                     (dense schedules only; empty when sparse)
     int off_mod = 0;   // 1        the modulus limbs (plain integer): the kernels load them from here into registers
     int off_sc0 = 0;   // 1        S(C[0][0]): lane 0 after the first S-box when it entered the permutation as zero (fresh sponge)
@@ -196,7 +197,7 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
     S.t = t; S.rate = P.rate; S.capacity = P.capacity; S.rf = rf; S.rp = rp; S.alpha = P.alpha;
 
     const FeVec& M = P.mds;
-    FeVec C((size_t)rf * t), Mpre = M, Cp0((size_t)t, F.zero()), pc((size_t)(rp > 0 ? rp : 1), F.zero());
+    FeVec C((size_t)rf * t), Mpre = M, Mpost = M, Cp0((size_t)t, F.zero()), pc((size_t)(rp > 0 ? rp : 1), F.zero());
     FeVec sp((size_t)(rp > 0 ? rp : 1) * (2 * t - 1), F.zero()), arkp;
     auto ark = [&](int r, int i) -> const Fe& { return P.ark[(size_t)r * t + i]; };
     for (int fr = 0; fr < rf; fr++) {
@@ -206,7 +207,8 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
     for (int k = 0; k < rp; k++)
         for (int i = 0; i < t; i++) arkp.push_back(ark(half + k, i));
 
-    bool sparse = allow_sparse && rp > 0 && t >= 2 && half >= 1 && rf > half;
+    // m00 = M[0][0] != 0: the lane-0 scale below divides by products of it
+    bool sparse = allow_sparse && rp > 0 && t >= 2 && half >= 1 && rf > half && !M[0].is_zero();
     if (sparse) {
         // backward factorisation  N_k = D_{k+1} * M = Sp_k * D_k,  D_rp = I
         FeVec D((size_t)t * t, F.zero());
@@ -246,9 +248,33 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
                 d[0] = F.zero();
             }
             FeVec post = detail::matvec(F, M, d, t);
-            if (rf > half)
-                for (int i = 0; i < t; i++) C[(size_t)half * t + i] = F.add(C[(size_t)half * t + i], post[i]);
-            else sparse = false;   // no later full round to absorb the folded constants
+            for (int i = 0; i < t; i++) C[(size_t)half * t + i] = F.add(C[(size_t)half * t + i], post[i]);
+            // Lane 0 is carried as L = lane0 / lam_k through the partial rounds: lam_0 = 1, lam_{k+1} = m00 * lam_k^alpha.  As
+            // S(lam*y) = lam^alpha * S(y), round k becomes L' = xi + (w_hat / lam_{k+1}) . s, s' = s + (v * lam_k^alpha) * xi with
+            // xi = S(L): the row's lane-0 coefficient is exactly one, which the kernels add instead of multiplying.  The constant
+            // entering lane 0 at round k is divided by lam_k; the first second-half full round takes lam_rp out again through its
+            // lane-0 constant and column 0 of its matrix (Mpost = M * diag(lam_rp^alpha, 1, ..., 1)).  Exact field algebra.
+            auto pow_alpha = [&](Fe b) {
+                Fe y = F.one();
+                for (u64 e = P.alpha; e; e >>= 1) {
+                    if (e & 1) y = F.mul(y, b);
+                    b = F.mul(b, b);
+                }
+                return y;
+            };
+            Fe lam = F.one();
+            for (int k = 0; k < rp; k++) {
+                Fe* row = &sp[(size_t)k * (2 * t - 1)];
+                const Fe la = pow_alpha(lam), next = F.mul(row[0], la), inv_next = F.inv(next);
+                row[0] = F.one();
+                for (int j = 1; j < t; j++) row[j] = F.mul(row[j], inv_next);
+                for (int j = 0; j < t - 1; j++) row[t + j] = F.mul(row[t + j], la);
+                if (k > 0) pc[k] = F.mul(pc[k], F.inv(lam));
+                lam = next;
+            }
+            C[(size_t)half * t] = F.mul(C[(size_t)half * t], F.inv(lam));
+            const Fe la = pow_alpha(lam);
+            for (int i = 0; i < t; i++) Mpost[(size_t)i * t] = F.mul(M[(size_t)i * t], la);
         }
     }
     if (!sparse) {
@@ -258,6 +284,7 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
             for (int i = 0; i < t; i++) C[(size_t)fr * t + i] = ark(r, i);
         }
         Mpre = M;
+        Mpost = M;
     }
     S.sparse = sparse ? 1 : 0;
 
@@ -269,6 +296,7 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
     S.off_c = push(C);
     S.off_m = push(M);
     S.off_mpre = push(Mpre);
+    push(Mpost);                   // at off_mpre + t*t (pos_full_matrix)
     S.off_cp0 = push(Cp0);
     S.off_pc = push(pc);
     S.off_sp = push(sp);

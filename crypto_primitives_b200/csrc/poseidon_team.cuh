@@ -21,7 +21,8 @@
 // S-box + one product).  BN254 Fr (8 + 57 rounds): 8*5 + 57*3 = 211 multiplication times per level instead of 268.
 // Values are exchanged through single-buffered shared-memory slots with one __syncthreads after each phase: a slot
 // written in phase p of a round is read only in the following phase and rewritten no earlier than phase p of the next
-// round, two barriers later.  Same schedule (poseidon_host.hpp) and field values as poseidon.cuh => identical outputs.
+// round, two barriers later.  Same schedule (poseidon_host.hpp) and field values as poseidon.cuh => identical outputs.  (Sparse
+// schedules carry lane 0 scaled and store m00 as one, so a = x here; the product is off the critical path and is kept.)
 // The phase functions are CPB_HD: tests/host runs them for w = 0..3 in sequence as the CPU model of the kernel.
 #pragma once
 #include "poseidon.cuh"
@@ -49,7 +50,6 @@ constexpr int kTeamThreads = 128;
 struct TeamRound {
     bool full, sparse_partial;
     int fr, k;            // index among the full rounds / among the partial rounds
-    bool last_first_half; // the full round whose matrix is Mpre and after which the first partial round starts
 };
 CPB_HD TeamRound team_round(const PoseidonDev& P, int r) {
     const int half = P.rf / 2;
@@ -58,7 +58,6 @@ CPB_HD TeamRound team_round(const PoseidonDev& P, int r) {
     R.sparse_partial = !R.full && P.sparse;
     R.fr = r < half ? r : r - P.rp;
     R.k = r - half;
-    R.last_first_half = R.full && r == half - 1;
     return R;
 }
 
@@ -130,7 +129,7 @@ CPB_HD void team_phase2(u32* s, const u32* t, int w, int lane, int r, const Pose
         u32 v[3][8];
 #pragma unroll
         for (int j = 0; j < 3; j++) ld_elem(v[j], team_slot(xb, TS_L0 + j, lane));
-        const u32* M = cs + 8 * ((R.last_first_half) ? P.off_mpre : P.off_m);
+        const u32* M = cs + 8 * (R.full ? pos_full_matrix(P, R.fr) : P.off_m);
         u32 d[8];
         fp_dot<F, 3>(d, v, M + 8 * 3 * w, pm);
         fp_copy(s, d);
