@@ -515,6 +515,21 @@ template <class F, int T, int XI> CPB_HD void fp_dot_unit(u32* r, const u32 (&a)
     for (int i = 0; i < 8; i++) r[i] = w[i];
 }
 
+// r = a + b mod p, fully reduced, for a < 2p (an output of the LAZY multiplier) and b in [0,p): a + b < 3p, brought to [0,p)
+// by two conditional subtractions, 2p then p.  Needs 3p < 2^256 (the F::LAZY5 fields).  r may alias a or b.
+template <class F> CPB_HD void fp_add_lazy(u32* r, const u32* a, const u32* b) {
+    static_assert(3 * ((u64)F::P(7) + 1) <= ((u64)1 << LIMB_BITS), "fp_add_lazy needs 3p < 2^256");
+    fp_add_noreduce(r, a, b);
+    u32 t[8];
+    t[0] = sub_cc(r[0], detail::p_shl<F>(1, 0));
+#pragma unroll
+    for (int i = 1; i < 8; i++) t[i] = subc_cc(r[i], detail::p_shl<F>(1, i));
+    u32 borrow = subc(0, 0);   // 0xffffffff when r < 2p
+#pragma unroll
+    for (int i = 0; i < 8; i++) r[i] = borrow ? r[i] : t[i];
+    fp_final_sub<F>(r);
+}
+
 
 // r = a*a/R mod p.  Dedicated squaring: the 28 cross products are computed once and doubled with
 // adds (the ALU pipe has slack, the multiply pipe does not), then the 8 diagonal squares are added

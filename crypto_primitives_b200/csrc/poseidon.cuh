@@ -115,6 +115,11 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
     constexpr bool LZ = F::LAZY5 && !detail::dot_needs_x<F, T + 1>() && T <= 4;
     static_assert(!F::LAZY5 || 100 * ((u64)F::P(7) + 1) <= 19 * ((u64)1 << LIMB_BITS), "LAZY5 needs p/2^256 <= 0.19");
     const bool lazy = LZ && CPB_SBOX5 && P.alpha == 5;
+    // Lane 1 is carried as a = w_hat . s through the partial rounds (poseidon_host.hpp).  Its coefficients follow S(c0) in the
+    // schedule (so PoseidonDev needs no field): per round [gamma, alpha, beta | v[2..T-1]], then the Mpre row and Cp0 entry that
+    // put lane 1 into that basis on entry.
+    const u32* lp = cs + 8 * (P.off_sc0 + 1);
+    const u32* lp_entry = lp + 8 * P.rp * (2 * T - 2);
     u32 n[T][8];
 #pragma unroll
     for (int i = 0; i < T; i++) fp_zero(n[i]);
@@ -134,11 +139,12 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
                 pos_rotl<T>(s);
             }
             const u32* rows = cs + 8 * pos_full_matrix(P, phase * half + q);
+            const bool entry = phase == 0 && q == cnt - 1;                                 // Mpre: row 1 of the split form
 #pragma unroll 1
             for (int i = 0; i < T; i++) {
                 u32 d[8];
                 fp_zero(d);
-                if ((need >> i) & 1u) fp_dot<F, T, LZ ? 1 : 0>(d, s, rows + 8 * T * i, pm);
+                if ((need >> i) & 1u) fp_dot<F, T, LZ ? 1 : 0>(d, s, (entry && i == 1) ? lp_entry : rows + 8 * T * i, pm);
 #pragma unroll
                 for (int k = 0; k + 1 < T; k++) fp_copy(n[k], n[k + 1]);
                 fp_copy(n[T - 1], d);
@@ -147,20 +153,24 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
             for (int i = 0; i < T; i++) fp_copy(s[i], n[i]);
         }
         if (phase == 0 && P.rp > 0) {
-            pos_add_vec<F, T>(s, cs + 8 * P.off_cp0);
-            const u32* row = cs + 8 * P.off_sp;
+#pragma unroll
+            for (int i = 0; i < T; i++) {                                  // Cp0, lane 1's entry in the w_hat_0 basis
+                u32 c[8];
+                ld_elem(c, i == 1 ? lp_entry + 8 * T : cs + 8 * (P.off_cp0 + i));
+                fp_add<F>(s[i], s[i], c);
+            }
+            const u32* row = lp;
             const u32* pc = cs + 8 * (P.off_pc + 1);
-            // Lane 0 is carried scaled (poseidon_host.hpp), so the row's coefficient of the S-box output y is one: the row is
-            // y + sum_{j>=1} w_j * s_j (fp_dot_unit), T-1 products instead of T.
+            // Lane 0 is carried scaled and lane 1 as a = w_hat . s (poseidon_host.hpp): the row is L' = y + a, additions only, and
+            // lane 1 moves on with one T-term dot a' = gamma*y + alpha*a + sum_{j>=2} beta_j*s_j over the state as it stands.
             // Lazy lane 0 (LZ): lane 0 lives in [0, 2p) from the constant
-            // addition to the end of the round.  With a, b < 2p the Montgomery product (a*b + M*p)/R is below p*(4p/R + 1) <= 2p,
-            // so x^2, x^4, x^5 need no conditional subtraction, nor does x = d + c (d, c < p).  Consumers: the row adds y < 2p
-            // to the (T-1)-term sum over canonical lanes, value < 2p + p*((T-1)*p/R + 1) < 4p, and returns a canonical d; the
-            // column products v_j * y are ordinary multiplications whose full operand y + p stays below 2^256 and whose results
-            // are reduced, so lanes 1.. stay canonical.  Saves 4 conditional subtractions (68 instructions) per partial round;
-            // bit-identical outputs.
+            // addition to the S-box output.  With a, b < 2p the Montgomery product (a*b + M*p)/R is below p*(4p/R + 1) <= 2p,
+            // so x^2, x^4, x^5 need no conditional subtraction, nor does x = d + c (d, c < p).  Consumers of y < 1.60p: the dot
+            // takes it as its one unreduced term (EX = 1) and returns a canonical a'; d = y + a < 2.60p is made canonical by two
+            // conditional subtractions (fp_add_lazy); the column products v_j * y are ordinary multiplications whose full operand
+            // y + p stays below 2^256 and whose results are reduced, so lanes 2.. stay canonical.  Bit-identical outputs.
 #pragma unroll 1
-            for (int k = 0; k < P.rp; k++, row += 8 * (2 * T - 1), pc += 8) {
+            for (int k = 0; k < P.rp; k++, row += 8 * (2 * T - 2), pc += 8) {
 #if CPB_SBOX5
                 if (P.alpha == 5) {                   // straight-line x^5
                     u32 x2[8];
@@ -171,38 +181,41 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
 #endif
                 if (alpha_zero) fp_one<F>(s[0]);
                 else pos_sbox<F>(s[0], P.alpha, top_bit, pm);
-                u32 d[8];
-                fp_dot_unit<F, T, LZ ? 2 : 1>(d, s, row + 8, pm);       // row = [one, w_hat[1..T-1]]
-                const u32* v = row + 8 * T;
+                u32 an[8];
+                fp_dot<F, T, LZ ? 1 : 0>(an, s, row, pm);                // row = [gamma, alpha, beta[2..T-1]]
+                if constexpr (LZ) fp_add_lazy<F>(s[1], s[0], s[1]);      // s[1] <- d = y + a
+                else fp_add<F>(s[1], s[0], s[1]);
+                const u32* v = row + 8 * T;                               // v[2..T-1]
                 if (T <= CPB_COL_UNROLL_MAX) {
 #pragma unroll
-                    for (int j = 1; j < T; j++) {
+                    for (int j = 2; j < T; j++) {
                         u32 c[8], tmp[8];
-                        ld_elem(c, v + 8 * (j - 1));
+                        ld_elem(c, v + 8 * (j - 2));
                         fp_mul<F>(tmp, s[0], c, pm);
                         fp_add<F>(s[j], s[j], tmp);
                     }
                 } else {
 #pragma unroll 1
-                    for (int j = 1; j < T; j++) {
+                    for (int j = 2; j < T; j++) {
                         u32 c[8], tmp[8];
-                        ld_elem(c, v + 8 * (j - 1));
+                        ld_elem(c, v + 8 * (j - 2));
                         fp_mul<F>(tmp, s[0], c, pm);
-                        fp_add<F>(s[1], s[1], tmp);
-                        fp_copy(tmp, s[1]);
+                        fp_add<F>(s[2], s[2], tmp);
+                        fp_copy(tmp, s[2]);                               // rotate lanes 2..T-1
 #pragma unroll
-                        for (int q = 1; q + 1 < T; q++) fp_copy(s[q], s[q + 1]);
+                        for (int q = 2; q + 1 < T; q++) fp_copy(s[q], s[q + 1]);
                         fp_copy(s[T - 1], tmp);
                     }
                 }
                 if (k + 1 < P.rp) {
                     u32 c[8];
                     ld_elem(c, pc);
-                    if (lazy) fp_add_noreduce(s[0], d, c);
-                    else fp_add<F>(s[0], d, c);
+                    if (lazy) fp_add_noreduce(s[0], s[1], c);
+                    else fp_add<F>(s[0], s[1], c);
                 } else {
-                    fp_copy(s[0], d);
+                    fp_copy(s[0], s[1]);
                 }
+                fp_copy(s[1], an);
             }
         }
     }

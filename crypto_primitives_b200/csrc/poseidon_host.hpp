@@ -8,7 +8,8 @@
 //    dense t x t MDS in all RF+RP rounds; here the RP partial rounds use the equivalent
 //    sparse form (1 row + 1 column per round) with round constants folded so that only lane 0
 //    receives a constant.  The rewrite is exact field algebra, so outputs are bit-identical;
-//    when a required (t-1)x(t-1) minor is singular the schedule falls back to the dense form.
+//    when a required (t-1)x(t-1) minor is singular, M[0][0] = 0, or a row's w_hat[1] is zero (the
+//    split loop carries lane 1 as w_hat . s and divides by it), the schedule falls back to the dense form.
 #pragma once
 #include "hostfp.hpp"
 
@@ -133,6 +134,8 @@ struct PoseidonSchedule {
     int off_arkp = 0;  // rp x t   original partial-round constants                     (dense schedules only; empty when sparse)
     int off_mod = 0;   // 1        the modulus limbs (plain integer): the kernels load them from here into registers
     int off_sc0 = 0;   // 1        S(C[0][0]): lane 0 after the first S-box when it entered the permutation as zero (fresh sponge)
+                       // then, at off_sc0 + 1 (sparse only): rp x (2t-2) per round [gamma, alpha, beta[2..t-1] | v[2..t-1]], then
+                       //          Mpre's row 1 (t) and Cp0's entry 1 for lane 1 carried as w_hat . s (pos_permute_split only)
     int n_elems = 0;
     std::vector<u64> consts;
 };
@@ -198,7 +201,7 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
 
     const FeVec& M = P.mds;
     FeVec C((size_t)rf * t), Mpre = M, Mpost = M, Cp0((size_t)t, F.zero()), pc((size_t)(rp > 0 ? rp : 1), F.zero());
-    FeVec sp((size_t)(rp > 0 ? rp : 1) * (2 * t - 1), F.zero()), arkp;
+    FeVec sp((size_t)(rp > 0 ? rp : 1) * (2 * t - 1), F.zero()), arkp, lp;
     auto ark = [&](int r, int i) -> const Fe& { return P.ark[(size_t)r * t + i]; };
     for (int fr = 0; fr < rf; fr++) {
         int r = fr < half ? fr : half + rp + (fr - half);
@@ -225,6 +228,7 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
                 for (int i = 0; i < m; i++) acc = F.add(acc, F.mul(N[(size_t)0 * t + (i + 1)], Minv[(size_t)i * m + j]));
                 sp[(size_t)k * (2 * t - 1) + 1 + j] = acc;
             }
+            if (sp[(size_t)k * (2 * t - 1) + 1].is_zero()) { sparse = false; break; }   // lane 1's basis change divides by w_hat[1]
             sp[(size_t)k * (2 * t - 1)] = N[0];   // m00 (row 0 of N equals row 0 of M)
             for (int i = 0; i < m; i++) sp[(size_t)k * (2 * t - 1) + t + i] = N[(size_t)(i + 1) * t + 0];
             for (auto& e : D) e = F.zero();
@@ -275,6 +279,37 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
             C[(size_t)half * t] = F.mul(C[(size_t)half * t], F.inv(lam));
             const Fe la = pow_alpha(lam);
             for (int i = 0; i < t; i++) Mpost[(size_t)i * t] = F.mul(M[(size_t)i * t], la);
+
+            // The split loop (pos_permute_split) carries lane 1 as a_k = w_hat_k . s (s = lanes 1..t-1, w_hat as scaled above) and
+            // lanes 2.. as they are.  With w_hat_k[1] != 0, s_1 = (a_k - sum_{j>=2} w_hat_k[j]*s_j) / w_hat_k[1], so partial round k
+            // (xi = S(L), L' = xi + a_k, s' = s + v_k*xi) needs no row product and updates lane 1 with one t-term dot:
+            //   a_{k+1} = w_hat_{k+1} . s' = gamma_k*xi + alpha_k*a_k + sum_{j>=2} beta_kj*s_j,
+            //   alpha_k = w_hat_{k+1}[1] / w_hat_k[1],  beta_kj = w_hat_{k+1}[j] - alpha_k*w_hat_k[j],  gamma_k = w_hat_{k+1} . v_k.
+            // w_hat_rp := e_1 makes a_rp = s_1: the state leaves the loop in the plain basis.  Entry: a_0 = w_hat_0 . (Mpre*y + Cp0)
+            // is folded into row 1 of Mpre and entry 1 of Cp0, stored separately because the merged loop and the team kernel
+            // still read the plain ones.  Per round [gamma, alpha, beta_2..t-1 | v_k[2..t-1]] (the dot's coefficients in the
+            // state's lane order), then the split form's Mpre row 1 (t) and Cp0 entry 1.  Exact field algebra.
+            const int q = 2 * t - 2;
+            lp.assign((size_t)rp * q + t + 1, F.zero());
+            for (int k = 0; k < rp; k++) {
+                const Fe* w = &sp[(size_t)k * (2 * t - 1)];                    // w[j] = w_hat_k[j] (j >= 1), v_k[j] = w[t - 1 + j]
+                FeVec wn((size_t)t, F.zero());
+                if (k + 1 < rp) for (int j = 1; j < t; j++) wn[j] = sp[(size_t)(k + 1) * (2 * t - 1) + j];
+                else wn[1] = F.one();
+                Fe* o = &lp[(size_t)k * q];
+                o[1] = F.mul(wn[1], F.inv(w[1]));
+                for (int j = 1; j < t; j++) o[0] = F.add(o[0], F.mul(wn[j], w[t - 1 + j]));
+                for (int j = 2; j < t; j++) {
+                    o[j] = F.sub(wn[j], F.mul(o[1], w[j]));
+                    o[t + j - 2] = w[t - 1 + j];
+                }
+            }
+            Fe* entry = &lp[(size_t)rp * q];
+            for (int j = 1; j < t; j++) {
+                const Fe w0 = sp[j];
+                for (int i = 0; i < t; i++) entry[i] = F.add(entry[i], F.mul(w0, Mpre[(size_t)j * t + i]));
+                entry[t] = F.add(entry[t], F.mul(w0, Cp0[j]));
+            }
         }
     }
     if (!sparse) {
@@ -315,6 +350,7 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
         }
         S.off_sc0 = push(FeVec(1, y));
     }
+    push(lp);                      // at off_sc0 + 1 (pos_permute_split); empty when dense
     S.n_elems = (int)(S.consts.size() / 4);
     return S;
 }

@@ -178,7 +178,7 @@ cpb_status launch_verify_ft(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, cons
 // the consumer) instead of a grid-wide barrier: a CTA starts level l as soon as ITS inputs exist.  Children are read
 // with ld.global.cg (L2): they were written by other SMs during this launch.  A CTA with no hashes left at a level has
 // none at any later level and exits.  All CTAs of the grid (<= 128) must be resident for the spins to end; they are
-// 128-thread CTAs with ~16 KB of shared memory on a 132-SM H100, and every spin is bounded (trap after ~4 s).
+// 128-thread CTAs with ≤ 29 KB of shared memory at t = 3 on a 132-SM H100, and every spin is bounded (trap after ~4 s).
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kMaxPeers = 16;
 struct ExchangeDev {
