@@ -8,7 +8,7 @@ and every compute call fails without an H100.
 """
 from . import _native
 from .fields import BLS12_381_FR, BLS12_377_FR, BN254_FR, JUBJUB_FR, FIELDS, Field
-from .sponge.poseidon import (PoseidonConfig, PoseidonSponge, absorb_squeeze_batch, find_poseidon_ark_and_mds,
+from .sponge.poseidon import (PoseidonConfig, PoseidonSponge, absorb_squeeze_batch, absorb_squeeze_ragged, find_poseidon_ark_and_mds,
                               get_default_poseidon_parameters)
 from .crh import poseidon as crh_poseidon
 from .crh import pedersen as crh_pedersen
@@ -18,4 +18,5 @@ from . import curves
 from . import merkle_tree
 
 __all__ = ["Field", "FIELDS", "BLS12_381_FR", "BN254_FR", "JUBJUB_FR", "BLS12_377_FR", "PoseidonConfig", "PoseidonSponge", "absorb_squeeze_batch",
+           "absorb_squeeze_ragged",
            "find_poseidon_ark_and_mds", "get_default_poseidon_parameters", "crh_poseidon", "crh_pedersen", "crh_bowe_hopwood", "commitment_pedersen", "curves", "merkle_tree"]

@@ -46,6 +46,14 @@ SIGNATURES = {
     "cpb_poseidon_sponge_batch_dev": (C.c_int, [vp, vp, C.c_size_t, vp, C.c_size_t, C.c_size_t, vp]),
     "cpb_merkle_poseidon_verify_batch": (C.c_int, [vp, vp, u64p, u64p, C.c_size_t, u64p, u64p, C.c_size_t, u64p, u8p, C.c_size_t]),
     "cpb_merkle_poseidon_verify_batch_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp]),
+    "cpb_poseidon_crh_ragged_batch": (C.c_int, [vp, u64p, u64p, u64p, C.c_size_t]),
+    "cpb_poseidon_crh_ragged_batch_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, vp]),
+    "cpb_poseidon_sponge_ragged_batch": (C.c_int, [vp, u64p, u64p, u64p, C.c_size_t, C.c_size_t]),
+    "cpb_poseidon_sponge_ragged_batch_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, C.c_size_t, vp]),
+    "cpb_merkle_poseidon_build_ragged": (C.c_int, [vp, vp, u64p, u64p, C.c_size_t, u64p, u64p]),
+    "cpb_merkle_poseidon_build_ragged_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, vp, vp, vp]),
+    "cpb_merkle_poseidon_verify_ragged_batch": (C.c_int, [vp, vp, u64p, u64p, u64p, u64p, u64p, C.c_size_t, u64p, u8p, C.c_size_t]),
+    "cpb_merkle_poseidon_verify_ragged_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp]),
     "cpb_poseidon_compress_batch": (C.c_int, [vp, u64p, u64p, C.c_size_t]),
     "cpb_poseidon_compress_batch_dev": (C.c_int, [vp, vp, vp, C.c_size_t, vp]),
     "cpb_merkle_poseidon_build": (C.c_int, [vp, vp, u64p, C.c_size_t, C.c_size_t, u64p, u64p]),

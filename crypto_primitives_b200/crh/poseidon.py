@@ -6,6 +6,7 @@ from __future__ import annotations
 import numpy as np
 
 from .. import _native as N
+from .. import ragged as R
 from ..sponge.poseidon import PoseidonConfig
 
 
@@ -33,7 +34,10 @@ class CRH:
 
     @staticmethod
     def evaluate_batch(parameters: PoseidonConfig, inputs, device: int = 0) -> np.ndarray:
-        """inputs (n, len, 4) -> (n, 4)."""
+        """inputs (n, len, 4) -> (n, 4).  A list of (L_i, 4) arrays whose lengths differ is hashed as a ragged batch, each input at
+        its own length (evaluate_ragged)."""
+        if R.is_ragged(inputs):
+            return CRH.evaluate_ragged(parameters, *R.pack(inputs), device)
         inp = np.ascontiguousarray(inputs, dtype=np.uint64)
         assert inp.ndim == 3 and inp.shape[2] == 4
         n, ln = inp.shape[0], inp.shape[1]
@@ -50,6 +54,32 @@ class CRH:
             out = torch.empty((n, 4), dtype=torch.int64, device=inputs.device)
         N.check(N.lib.cpb_poseidon_crh_batch_dev(parameters.context(inputs.device.index), inputs.data_ptr(), ln,
                                                  out.data_ptr(), n, _stream_ptr()))
+        return out
+
+    @staticmethod
+    def evaluate_ragged(parameters: PoseidonConfig, values, offsets, device: int = 0) -> np.ndarray:
+        """n = len(offsets) - 1 inputs of different lengths: input i = values[offsets[i] .. offsets[i+1]) -> (n, 4).
+        Offsets that decrease raise ValueError."""
+        vals, off = R.as_arrays(values, offsets)
+        n = off.shape[0] - 1
+        out = np.empty((n, 4), dtype=np.uint64)
+        if n:
+            R.check(N.lib.cpb_poseidon_crh_ragged_batch(parameters.context(device), _p(vals), _p(off), _p(out), n))
+        return out
+
+    @staticmethod
+    def evaluate_ragged_dev(parameters: PoseidonConfig, values, offsets, out=None):
+        """evaluate_ragged on torch CUDA tensors (values int64 (m, 4), offsets int64 (n + 1,)), on the current stream.  The
+        offsets are not checked: they must not decrease (a decreasing pair hashes as an empty input)."""
+        import torch
+        assert values.is_cuda and values.is_contiguous() and values.dtype == torch.int64 and values.shape[-1] == 4
+        assert offsets.is_cuda and offsets.is_contiguous() and offsets.dtype == torch.int64 and offsets.dim() == 1
+        assert offsets.device == values.device
+        n = offsets.numel() - 1
+        if out is None:
+            out = torch.empty((n, 4), dtype=torch.int64, device=values.device)
+        R.check(N.lib.cpb_poseidon_crh_ragged_batch_dev(parameters.context(values.device.index), values.data_ptr(), offsets.data_ptr(),
+                                                        out.data_ptr(), n, _stream_ptr()))
         return out
 
 

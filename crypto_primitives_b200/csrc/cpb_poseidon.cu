@@ -108,6 +108,10 @@ CPB_POS_WIDTHS(CPB_POS_EXTERN, Bls12_381_Fr)
 CPB_POS_WIDTHS(CPB_POS_EXTERN, Bn254_Fr)
 CPB_POS_WIDTHS(CPB_POS_EXTERN, Jubjub_Fr)
 CPB_POS_WIDTHS(CPB_POS_EXTERN, Bls12_377_Fr)
+CPB_POS_WIDTHS(CPB_POS_EXTERN_RAGGED, Bls12_381_Fr)
+CPB_POS_WIDTHS(CPB_POS_EXTERN_RAGGED, Bn254_Fr)
+CPB_POS_WIDTHS(CPB_POS_EXTERN_RAGGED, Jubjub_Fr)
+CPB_POS_WIDTHS(CPB_POS_EXTERN_RAGGED, Bls12_377_Fr)
 CPB_POS_EXTERN_TEAM(Bls12_381_Fr)
 CPB_POS_EXTERN_TEAM(Bn254_Fr)
 CPB_POS_EXTERN_TEAM(Jubjub_Fr)
@@ -369,6 +373,162 @@ size_t count_launches(const cpb_poseidon_ctx* node, size_t n) {
 }
 
 bool pow2_gt1(size_t n) { return n > 1 && (n & (n - 1)) == 0; }
+
+// ------------------------------------------------------------------------------ ragged batches
+// Counting sort of the items by absorb-permutation count (ragged_key, poseidon.cuh) into order[n]: a histogram, an exclusive
+// scan, a scatter.  Each CTA of the histogram and scatter kernels owns kSortBlock * kSortItems consecutive items; the scatter
+// reserves one slice per bucket with one global atomic, so items of a bucket stay in CTA-sized runs of nearby inputs.
+constexpr int kSortBlock = 256, kSortItems = 8;
+
+struct RaggedHeader {
+    unsigned hist[kRaggedBuckets];
+    unsigned cursor[kRaggedBuckets];
+    unsigned starts[kRaggedBuckets + 1];
+    unsigned range[4];                  // ragged_ranges: [single begin, end, sponge begin, end)
+};
+
+// counter[key] += 1 for every calling lane, one shared atomic per distinct key of the warp; returns this lane's old count.
+__device__ __forceinline__ unsigned warp_aggregated_inc(unsigned* counter, int key) {
+    const unsigned peers = __match_any_sync(__activemask(), key);
+    const int lane = threadIdx.x & 31, leader = __ffs(peers) - 1;
+    unsigned base = 0;
+    if (lane == leader) base = atomicAdd(counter + key, (unsigned)__popc(peers));
+    base = __shfl_sync(peers, base, leader);
+    return base + __popc(peers & ((1u << lane) - 1u));
+}
+
+__global__ void __launch_bounds__(kSortBlock) k_ragged_hist(const u64* __restrict__ offsets, long n, int rate, unsigned* __restrict__ hist) {
+    __shared__ unsigned h[kRaggedBuckets];
+    for (int b = threadIdx.x; b < kRaggedBuckets; b += kSortBlock) h[b] = 0;
+    __syncthreads();
+    const long first = (long)blockIdx.x * (kSortBlock * kSortItems) + threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < kSortItems; k++) {
+        const long i = first + (long)k * kSortBlock;
+        if (i < n) warp_aggregated_inc(h, ragged_key(ragged_span(offsets, i, n).len, rate));
+    }
+    __syncthreads();
+    for (int b = threadIdx.x; b < kRaggedBuckets; b += kSortBlock)
+        if (h[b]) atomicAdd(hist + b, h[b]);
+}
+
+__global__ void k_ragged_scan(RaggedHeader* H, int single) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    ragged_scan(H->hist, H->starts);
+    for (int b = 0; b < kRaggedBuckets; b++) H->cursor[b] = H->starts[b];
+    ragged_ranges(H->starts, single != 0, H->range);
+}
+
+__global__ void __launch_bounds__(kSortBlock) k_ragged_scatter(const u64* __restrict__ offsets, long n, int rate, unsigned* __restrict__ cursor,
+                                                               unsigned* __restrict__ order) {
+    __shared__ unsigned h[kRaggedBuckets], base[kRaggedBuckets];
+    for (int b = threadIdx.x; b < kRaggedBuckets; b += kSortBlock) h[b] = 0;
+    __syncthreads();
+    const long first = (long)blockIdx.x * (kSortBlock * kSortItems) + threadIdx.x;
+    int key[kSortItems];
+    unsigned slot[kSortItems];
+#pragma unroll
+    for (int k = 0; k < kSortItems; k++) {
+        const long i = first + (long)k * kSortBlock;
+        key[k] = 0;
+        slot[k] = 0;
+        if (i < n) {
+            key[k] = ragged_key(ragged_span(offsets, i, n).len, rate);
+            slot[k] = warp_aggregated_inc(h, key[k]);
+        }
+    }
+    __syncthreads();
+    for (int b = threadIdx.x; b < kRaggedBuckets; b += kSortBlock) base[b] = h[b] ? atomicAdd(cursor + b, h[b]) : 0u;
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < kSortItems; k++) {
+        const long i = first + (long)k * kSortBlock;
+        if (i < n) order[base[key[k]] + slot[k]] = (unsigned)i;
+    }
+}
+
+// CPB_RAGGED_ORDER=0 (read once) hashes ragged batches in input order with one sponge launch and no ordering step.  It exists
+// only to measure what the ordering buys (tools/perf_ragged.py); results are the same either way.
+bool ragged_order_enabled() {
+    static int v = -1;
+    if (v < 0) {
+        const char* e = getenv("CPB_RAGGED_ORDER");
+        v = (e && *e && atoi(e) == 0) ? 0 : 1;
+    }
+    return v != 0;
+}
+
+static cpb_status hash_ragged(cpb_poseidon_ctx* c, const u32* values, u64 vbase, const u64* offsets, const unsigned* order,
+                              const unsigned* ranges, u32* out, size_t n_out, size_t n, bool single, cudaStream_t st) {
+    CPB_FOR_FIELD(launch_crh_ragged_ft, c, values, vbase, offsets, order, ranges, out, n_out, n, single, st)
+    return fail(CPB_UNSUPPORTED, "state width t=%d is not built (this library: t = 2..9)", c->dev.t);
+}
+
+static cpb_status order_ragged(const u64* offsets, size_t n, int rate, bool single, RaggedHeader* H, unsigned* order, cudaStream_t st) {
+    const unsigned grid = (unsigned)((n + kSortBlock * kSortItems - 1) / (kSortBlock * kSortItems));
+    CPB_CUDA(cudaMemsetAsync(H->hist, 0, sizeof(H->hist), st));
+    k_ragged_hist<<<grid, kSortBlock, 0, st>>>(offsets, (long)n, rate, H->hist);
+    CPB_CUDA(cudaGetLastError());
+    k_ragged_scan<<<1, 32, 0, st>>>(H, single ? 1 : 0);
+    CPB_CUDA(cudaGetLastError());
+    k_ragged_scatter<<<grid, kSortBlock, 0, st>>>(offsets, (long)n, rate, H->cursor, order);
+    CPB_CUDA(cudaGetLastError());
+    return CPB_OK;
+}
+
+// n sponges over a ragged batch (device pointers): values[offsets[i] - vbase ..] -> out[i * n_out ..].  Ordering scratch comes from
+// the stream-ordered pool (keep_pool_memory), so nothing here synchronises the host.
+cpb_status launch_crh_ragged(cpb_poseidon_ctx* c, const u32* values, u64 vbase, const u64* offsets, u32* out, size_t n, size_t n_out,
+                             cudaStream_t st) {
+    if (n == 0 || n_out == 0) return CPB_OK;
+    if (n >= ((size_t)1 << 32)) return fail(CPB_BAD_LENGTH, "a ragged batch holds fewer than 2^32 inputs (got %zu)", n);
+    const bool single = n_out <= (size_t)c->dev.rate && c->dev.cap >= 1;
+    if (!ragged_order_enabled()) return hash_ragged(c, values, vbase, offsets, nullptr, nullptr, out, n_out, n, false, st);
+    const size_t hdr = (sizeof(RaggedHeader) + 255) & ~(size_t)255;
+    char* tmp = nullptr;
+    CPB_CUDA(cudaMallocAsync((void**)&tmp, hdr + n * sizeof(unsigned), st));
+    RaggedHeader* H = reinterpret_cast<RaggedHeader*>(tmp);
+    unsigned* order = reinterpret_cast<unsigned*>(tmp + hdr);
+    cpb_status rc = order_ragged(offsets, n, c->dev.rate, single, H, order, st);
+    if (rc == CPB_OK) rc = hash_ragged(c, values, vbase, offsets, order, H->range, out, n_out, n, single, st);
+    cudaFreeAsync(tmp, st);
+    return rc;
+}
+
+cpb_status launch_verify_ragged(cpb_poseidon_ctx* c, cpb_poseidon_ctx* node, const u32* root, const u32* values, u64 vbase, const u64* offsets,
+                                const u32* siblings, const u32* paths, int plen, const unsigned long long* indexes, unsigned char* ok,
+                                size_t n, cudaStream_t st) {
+    if (n == 0) return CPB_OK;
+    if (n >= ((size_t)1 << 32)) return fail(CPB_BAD_LENGTH, "a ragged batch holds fewer than 2^32 inputs (got %zu)", n);
+    CPB_FOR_FIELD(launch_verify_ragged_ft, c, node, root, values, vbase, offsets, siblings, paths, plen, indexes, ok, n, st)
+    return fail(CPB_UNSUPPORTED, "state width t=%d is not built (this library: t = 2..9)", c->dev.t);
+}
+
+// Host forms: offsets must not decrease (the _dev forms take that as a precondition and read a decreasing pair as empty).
+cpb_status check_offsets(const uint64_t* offsets, size_t n) {
+    for (size_t i = 0; i < n; i++)
+        if (offsets[i + 1] < offsets[i])
+            return fail(CPB_BAD_LENGTH, "offsets decrease at input %zu (%llu > %llu)", i, (unsigned long long)offsets[i],
+                        (unsigned long long)offsets[i + 1]);
+    if (n >= ((size_t)1 << 32)) return fail(CPB_BAD_LENGTH, "a ragged batch holds fewer than 2^32 inputs (got %zu)", n);
+    return CPB_OK;
+}
+
+// Copies a ragged host batch into `buf`: the n + 1 offsets at d_off, then values[offsets[0] .. offsets[n]) at d_val (so the
+// device values start at index vbase = offsets[0]).  `front` bytes at the start of buf are left to the caller.
+cpb_status stage_ragged(Scratch& buf, size_t front, const uint64_t* values, const uint64_t* offsets, size_t n, cudaStream_t st,
+                        u64*& d_off, u32*& d_val) {
+    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
+    const size_t b_off = (n + 1) * 8, b_val = (size_t)(offsets[n] - offsets[0]) * 32;
+    const size_t o_off = up(front), o_val = o_off + up(b_off);
+    CPB_TRY(buf.reserve(o_val + (b_val ? b_val : 32)));
+    char* d = (char*)buf.ptr;
+    d_off = (u64*)(d + o_off);
+    d_val = (u32*)(d + o_val);
+    CPB_CUDA(cudaMemcpyAsync(d_off, offsets, b_off, cudaMemcpyHostToDevice, st));
+    if (b_val) CPB_CUDA(cudaMemcpyAsync(d_val, values + 4 * offsets[0], b_val, cudaMemcpyHostToDevice, st));
+    return CPB_OK;
+}
 
 }  // namespace cpb
 
@@ -787,6 +947,143 @@ cpb_status cpb_merkle_poseidon_build(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* n
     MerkleHost H;
     H.leaves = (const u32*)leaves; H.leaf_nodes = (u32*)leaf_nodes; H.nodes = (u32*)non_leaf_nodes;
     CPB_TRY(merkle_build_streams(leaf, node, (const u32*)leaf->s_in.ptr, leaf_len, n, (u32*)leaf->s_out.ptr, (u32*)leaf->s_aux.ptr, st, &H));
+    CPB_CUDA(cudaStreamSynchronize(st));
+    return CPB_OK;
+    });
+}
+
+// ---- ragged batches: input i is values[offsets[i] .. offsets[i+1])
+cpb_status cpb_poseidon_sponge_ragged_batch_dev(cpb_poseidon_ctx* c, const uint64_t* values, const uint64_t* offsets, uint64_t* out,
+                                                size_t n_squeeze, size_t n, void* stream) {
+    return cpb::guarded([&]() -> cpb_status {
+    CPB_TRY(check_ctx(c));
+    DeviceGuard g(c->device);
+    return launch_crh_ragged(c, (const u32*)values, 0, offsets, (u32*)out, n, n_squeeze, (cudaStream_t)stream);
+    });
+}
+cpb_status cpb_poseidon_crh_ragged_batch_dev(cpb_poseidon_ctx* c, const uint64_t* values, const uint64_t* offsets, uint64_t* out, size_t n,
+                                             void* stream) {
+    return cpb_poseidon_sponge_ragged_batch_dev(c, values, offsets, out, 1, n, stream);
+}
+cpb_status cpb_poseidon_sponge_ragged_batch(cpb_poseidon_ctx* c, const uint64_t* values, const uint64_t* offsets, uint64_t* out,
+                                            size_t n_squeeze, size_t n) {
+    return cpb::guarded([&]() -> cpb_status {
+    CPB_TRY(check_ctx(c));
+    if (n == 0 || n_squeeze == 0) return CPB_OK;
+    if (!offsets || !out) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(check_offsets(offsets, n));
+    if (!values && offsets[n] != offsets[0]) return fail(CPB_NULL_POINTER, "null values");
+    std::lock_guard<std::mutex> lk(c->mu);
+    DeviceGuard g(c->device);
+    u64* d_off = nullptr;
+    u32* d_val = nullptr;
+    CPB_TRY(stage_ragged(c->s_in, 0, values, offsets, n, c->stream, d_off, d_val));
+    CPB_TRY(c->s_out.reserve(n * n_squeeze * 32));
+    CPB_TRY(launch_crh_ragged(c, d_val, offsets[0], d_off, (u32*)c->s_out.ptr, n, n_squeeze, c->stream));
+    CPB_CUDA(cudaMemcpyAsync(out, c->s_out.ptr, n * n_squeeze * 32, cudaMemcpyDeviceToHost, c->stream));
+    CPB_CUDA(cudaStreamSynchronize(c->stream));
+    return CPB_OK;
+    });
+}
+cpb_status cpb_poseidon_crh_ragged_batch(cpb_poseidon_ctx* c, const uint64_t* values, const uint64_t* offsets, uint64_t* out, size_t n) {
+    return cpb_poseidon_sponge_ragged_batch(c, values, offsets, out, 1, n);
+}
+
+static cpb_status check_tree_ctxs(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, size_t n) {
+    CPB_TRY(check_ctx(leaf));
+    CPB_TRY(check_ctx(node));
+    if (leaf->device != node->device || leaf->field_id != node->field_id)
+        return fail(CPB_BAD_PARAMS, "leaf and node contexts must share device and field");
+    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
+    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    return CPB_OK;
+}
+
+// The ragged leaf hash, then the from-digests build (subtree streams and tree-top kernel included).
+cpb_status cpb_merkle_poseidon_build_ragged_dev(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, const uint64_t* values,
+                                                const uint64_t* offsets, size_t n, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes,
+                                                void* stream) {
+    return cpb::guarded([&]() -> cpb_status {
+    CPB_TRY(check_tree_ctxs(leaf, node, n));
+    DeviceGuard g(leaf->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    CPB_TRY(launch_crh_ragged(leaf, (const u32*)values, 0, offsets, (u32*)leaf_nodes, n, 1, st));
+    return merkle_build_streams(node, node, nullptr, 0, n, (u32*)leaf_nodes, (u32*)non_leaf_nodes, st);
+    });
+}
+cpb_status cpb_merkle_poseidon_build_ragged(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, const uint64_t* values, const uint64_t* offsets,
+                                            size_t n, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes) {
+    return cpb::guarded([&]() -> cpb_status {
+    CPB_TRY(check_tree_ctxs(leaf, node, n));
+    if (!offsets || !leaf_nodes || !non_leaf_nodes) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(check_offsets(offsets, n));
+    if (!values && offsets[n] != offsets[0]) return fail(CPB_NULL_POINTER, "null values");
+    std::lock_guard<std::mutex> lk(leaf->mu);
+    DeviceGuard g(leaf->device);
+    cudaStream_t st = leaf->stream;
+    u64* d_off = nullptr;
+    u32* d_val = nullptr;
+    CPB_TRY(stage_ragged(leaf->s_in, 0, values, offsets, n, st, d_off, d_val));
+    CPB_TRY(leaf->s_out.reserve(n * 32));
+    CPB_TRY(leaf->s_aux.reserve((n - 1) * 32));
+    CPB_TRY(launch_crh_ragged(leaf, d_val, offsets[0], d_off, (u32*)leaf->s_out.ptr, n, 1, st));
+    MerkleHost H;                        // no leaves to copy in: the subtree streams copy the digests and levels out
+    H.leaf_nodes = (u32*)leaf_nodes; H.nodes = (u32*)non_leaf_nodes;
+    CPB_TRY(merkle_build_streams(node, node, nullptr, 0, n, (u32*)leaf->s_out.ptr, (u32*)leaf->s_aux.ptr, st, &H));
+    CPB_CUDA(cudaStreamSynchronize(st));
+    return CPB_OK;
+    });
+}
+
+static cpb_status check_verify_ctxs(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, size_t path_len) {
+    CPB_TRY(check_ctx(leaf));
+    CPB_TRY(check_ctx(node));
+    if (leaf->device != node->device || leaf->field_id != node->field_id || leaf->dev.t != node->dev.t)
+        return fail(CPB_UNSUPPORTED, "leaf and node contexts must share device, field and state width");
+    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    if (path_len > 62) return fail(CPB_BAD_PARAMS, "path too long");
+    return CPB_OK;
+}
+cpb_status cpb_merkle_poseidon_verify_ragged_batch_dev(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, const uint64_t* root,
+                                                       const uint64_t* values, const uint64_t* offsets, const uint64_t* leaf_sibling_hashes,
+                                                       const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes,
+                                                       uint8_t* ok, size_t n, void* stream) {
+    return cpb::guarded([&]() -> cpb_status {
+    CPB_TRY(check_verify_ctxs(leaf, node, path_len));
+    DeviceGuard g(leaf->device);
+    return launch_verify_ragged(leaf, node, (const u32*)root, (const u32*)values, 0, offsets, (const u32*)leaf_sibling_hashes,
+                                (const u32*)auth_paths, (int)path_len, (const unsigned long long*)leaf_indexes, ok, n, (cudaStream_t)stream);
+    });
+}
+cpb_status cpb_merkle_poseidon_verify_ragged_batch(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, const uint64_t* root,
+                                                   const uint64_t* values, const uint64_t* offsets, const uint64_t* leaf_sibling_hashes,
+                                                   const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes, uint8_t* ok,
+                                                   size_t n) {
+    return cpb::guarded([&]() -> cpb_status {
+    CPB_TRY(check_verify_ctxs(leaf, node, path_len));
+    if (n == 0) return CPB_OK;
+    if (!root || !offsets || !leaf_sibling_hashes || (!auth_paths && path_len) || !leaf_indexes || !ok)
+        return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(check_offsets(offsets, n));
+    if (!values && offsets[n] != offsets[0]) return fail(CPB_NULL_POINTER, "null values");
+    std::lock_guard<std::mutex> lk(leaf->mu);
+    DeviceGuard g(leaf->device);
+    cudaStream_t st = leaf->stream;
+    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
+    const size_t b_sib = n * 32, b_path = n * path_len * 32, b_idx = n * 8;
+    const size_t o_sib = 256, o_path = o_sib + up(b_sib), o_idx = o_path + up(b_path), front = o_idx + up(b_idx);
+    u64* d_off = nullptr;
+    u32* d_val = nullptr;
+    CPB_TRY(stage_ragged(leaf->s_in, front, values, offsets, n, st, d_off, d_val));    // the fixed-size arrays go in front
+    CPB_TRY(leaf->s_out.reserve(n));
+    char* d = (char*)leaf->s_in.ptr;
+    CPB_CUDA(cudaMemcpyAsync(d, root, 32, cudaMemcpyHostToDevice, st));
+    CPB_CUDA(cudaMemcpyAsync(d + o_sib, leaf_sibling_hashes, b_sib, cudaMemcpyHostToDevice, st));
+    if (b_path) CPB_CUDA(cudaMemcpyAsync(d + o_path, auth_paths, b_path, cudaMemcpyHostToDevice, st));
+    CPB_CUDA(cudaMemcpyAsync(d + o_idx, leaf_indexes, b_idx, cudaMemcpyHostToDevice, st));
+    CPB_TRY(launch_verify_ragged(leaf, node, (const u32*)d, d_val, offsets[0], d_off, (const u32*)(d + o_sib), (const u32*)(d + o_path),
+                                 (int)path_len, (const unsigned long long*)(d + o_idx), (uint8_t*)leaf->s_out.ptr, n, st));
+    CPB_CUDA(cudaMemcpyAsync(ok, leaf->s_out.ptr, n, cudaMemcpyDeviceToHost, st));
     CPB_CUDA(cudaStreamSynchronize(st));
     return CPB_OK;
     });

@@ -409,4 +409,49 @@ CPB_HD bool pos_verify_path(const u32* leaf, long leaf_len, const u32* sibling, 
     return fp_eq(cur, r);
 }
 
+// ---- ragged batches: input i is values[offsets[i] .. offsets[i+1]), n + 1 offsets, offsets[0] not necessarily 0.
+// The hash launches walk the items sorted by their absorb-permutation count (a counting sort, cpb_poseidon.cu), so that a warp
+// runs items of one length class instead of as many permutations as its longest input.  Keys are clamped at kRaggedBuckets:
+// inputs of kRaggedBuckets or more blocks share the last bucket, and warps there may diverge.
+constexpr int kRaggedBuckets = 64;
+
+// Item i's slot range, clamped to [offsets[0], offsets[n]): a decreasing pair, or one outside that window, is an empty input, so
+// no thread reads outside the caller's values whatever the offsets hold.
+struct RaggedSpan {
+    u64 lo;
+    long len;
+};
+CPB_HD RaggedSpan ragged_span(const u64* offsets, long i, long n) {
+    const u64 a = offsets[0], b = offsets[n];
+    u64 lo = offsets[i], hi = offsets[i + 1];
+    if (lo < a) lo = a;
+    if (hi > b) hi = b;
+    if (hi <= lo) return RaggedSpan{a, 0};
+    return RaggedSpan{lo, (long)(hi - lo)};
+}
+// Absorb permutations of a `len`-element input (pos_sponge: an empty input still costs one) and its sort key, 0 .. kRaggedBuckets-1.
+CPB_HD long ragged_blocks(long len, int rate) { return len <= rate ? 1 : (len + rate - 1) / rate; }
+CPB_HD int ragged_key(long len, int rate) {
+    const long b = ragged_blocks(len, rate);
+    return (int)(b < kRaggedBuckets ? b : kRaggedBuckets) - 1;
+}
+// Exclusive scan of the key histogram: bucket b occupies order[starts[b] .. starts[b+1]); starts[kRaggedBuckets] = n.
+CPB_HD void ragged_scan(const unsigned* hist, unsigned* starts) {
+    unsigned s = 0;
+    for (int b = 0; b < kRaggedBuckets; b++) {
+        starts[b] = s;
+        s += hist[b];
+    }
+    starts[kRaggedBuckets] = s;
+}
+// The two hash launches' slices of `order`: range[0..1] for the one-permutation kernel (bucket 0, when the squeeze fits one
+// permutation too), range[2..3] for the general sponge kernel (everything else).
+CPB_HD void ragged_ranges(const unsigned* starts, bool single, unsigned* range) {
+    const unsigned split = single ? starts[1] : 0u;
+    range[0] = 0;
+    range[1] = split;
+    range[2] = split;
+    range[3] = starts[kRaggedBuckets];
+}
+
 }  // namespace cpb

@@ -1,6 +1,6 @@
 // poseidon_kernels.cuh -- Poseidon kernel templates, the context struct and the launch wrappers.
 // Included by cpb_poseidon.cu (C-ABI, dispatch) and by the per-field instantiation units
-// poseidon_inst_*.cu, which exist only so that nvcc can compile the (field, width) grid in parallel.
+// poseidon_inst_*.cu and poseidon_ragged_*.cu, which exist only so that nvcc can compile the (field, width) grid in parallel.
 #pragma once
 #include <mutex>
 
@@ -164,6 +164,98 @@ cpb_status launch_verify_ft(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, cons
     CPB_TRY(grid_for(k_poseidon_verify_paths<F, T>, smem, leaf->sms, (long)n, grid));
     k_poseidon_verify_paths<F, T><<<grid, kBlock, smem, st>>>(leaf->dev, leaf->d_consts, node->dev, node->d_consts, root, leaves,
                                                               (long)leaf_len, siblings, paths, plen, indexes, ok, (long)n);
+    CPB_CUDA(cudaGetLastError());
+    return CPB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Ragged batches (poseidon.cuh: ragged_span): item i hashes values[offsets[i] - vbase ..] at its own length and writes out[i].
+// Slot j of [range[0], range[1]) is item order[j]; order == nullptr walks the items in input order and range == nullptr is
+// [0, n).  The range lives in device memory (written by the ordering kernels), so the grid covers n slots and a CTA wholly past
+// the end of its range exits before staging.  One item per thread, no grid-stride loop: nothing but the item's own pointers stays
+// live across the hash, which keeps the t = 3 kernels at the uniform kernels' 96 registers.
+// SINGLE: every item of the range is one permutation (len <= rate, n_out <= rate, capacity >= 1): pos_hash_single.
+// ---------------------------------------------------------------------------------------------------------------
+template <class F, int T, bool SINGLE>
+__global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
+k_poseidon_crh_ragged(PoseidonDev P, const u32* __restrict__ consts, const u32* __restrict__ values, u64 vbase,
+                      const u64* __restrict__ offsets, const unsigned* __restrict__ order, const unsigned* __restrict__ range,
+                      u32* __restrict__ out, long n, long n_out) {
+    extern __shared__ __align__(16) u32 cs[];
+    __shared__ __align__(8) unsigned long long mbar;
+    const long begin = range ? (long)range[0] : 0, end = range ? (long)range[1] : n;
+    if (begin + (long)blockIdx.x * blockDim.x >= end) return;
+    tma_stage_to_smem(cs, consts, (unsigned)P.n_elems * 32u, &mbar);
+    const long j = begin + (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= end) return;
+    const u32* ct = cs + (int)threadIdx.x * P.zero;
+    u32 pm[8];
+    ld_elem(pm, ct + 8 * P.off_mod);
+    const long i = order ? (long)order[j] : j;
+    const RaggedSpan sp = ragged_span(offsets, i, n);
+    const u32* in = values + 8 * (sp.lo - vbase);
+    if constexpr (SINGLE) pos_hash_single<F, T>(out + 8 * n_out * i, (int)n_out, in, (int)sp.len, P, ct, pm);
+    else pos_sponge<F, T>(out + 8 * n_out * i, n_out, in, sp.len, P, ct, pm);
+}
+
+template <class K> cpb_status grid_ragged(K kernel, size_t smem, size_t n, int& grid) {
+    int occ = 0;
+    CPB_TRY(configure_kernel(kernel, smem, kBlock, occ));
+    grid = (int)((n + kBlock - 1) / kBlock);          // n < 2^32 (checked by the caller)
+    return CPB_OK;
+}
+
+// The two hash launches over the ordered items (or one sponge launch in input order when order == nullptr; range_* then unused).
+template <class F, int T>
+cpb_status launch_crh_ragged_ft(cpb_poseidon_ctx* c, const u32* values, u64 vbase, const u64* offsets, const unsigned* order,
+                                const unsigned* ranges, u32* out, size_t n_out, size_t n, bool single, cudaStream_t st) {
+    size_t smem = (size_t)c->dev.n_elems * 32;
+    int grid = 1;
+    if (order && single) {
+        CPB_TRY(grid_ragged(k_poseidon_crh_ragged<F, T, true>, smem, n, grid));
+        k_poseidon_crh_ragged<F, T, true><<<grid, kBlock, smem, st>>>(c->dev, c->d_consts, values, vbase, offsets, order, ranges, out,
+                                                                      (long)n, (long)n_out);
+        CPB_CUDA(cudaGetLastError());
+    }
+    CPB_TRY(grid_ragged(k_poseidon_crh_ragged<F, T, false>, smem, n, grid));
+    k_poseidon_crh_ragged<F, T, false><<<grid, kBlock, smem, st>>>(c->dev, c->d_consts, values, vbase, offsets, order,
+                                                                   order ? ranges + 2 : nullptr, out, (long)n, (long)n_out);
+    CPB_CUDA(cudaGetLastError());
+    return CPB_OK;
+}
+
+// Path::verify with each leaf at its own length; no ordering: a path's cost is dominated by its plen + 1 compressions.
+template <class F, int T>
+__global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
+k_poseidon_verify_paths_ragged(PoseidonDev PL, const u32* __restrict__ consts_l, PoseidonDev PN, const u32* __restrict__ consts_n,
+                               const u32* __restrict__ root, const u32* __restrict__ values, u64 vbase, const u64* __restrict__ offsets,
+                               const u32* __restrict__ siblings, const u32* __restrict__ paths, int plen,
+                               const unsigned long long* __restrict__ indexes, unsigned char* __restrict__ ok, long n) {
+    extern __shared__ __align__(16) u32 cs[];
+    __shared__ __align__(8) unsigned long long mbar[2];
+    u32* csn = cs + 8 * PL.n_elems;
+    tma_stage_to_smem(cs, consts_l, (unsigned)PL.n_elems * 32u, &mbar[0]);
+    tma_stage_to_smem(csn, consts_n, (unsigned)PN.n_elems * 32u, &mbar[1]);
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int z = (int)threadIdx.x * PL.zero;
+    u32 pm[8];
+    ld_elem(pm, cs + z + 8 * PL.off_mod);
+    const RaggedSpan sp = ragged_span(offsets, i, n);
+    ok[i] = pos_verify_path<F, T>(values + 8 * (sp.lo - vbase), sp.len, siblings + 8 * i, paths + 8 * (long)plen * i, plen, indexes[i],
+                                  root, PL, cs + z, PN, csn + z, pm) ? 1 : 0;
+}
+
+template <class F, int T>
+cpb_status launch_verify_ragged_ft(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, const u32* root, const u32* values, u64 vbase,
+                                   const u64* offsets, const u32* siblings, const u32* paths, int plen, const unsigned long long* indexes,
+                                   unsigned char* ok, size_t n, cudaStream_t st) {
+    size_t smem = ((size_t)leaf->dev.n_elems + node->dev.n_elems) * 32;
+    if (smem > 200 * 1024) return fail(CPB_UNSUPPORTED, "round schedules (%zu B) exceed shared memory", smem);
+    int grid = 1;
+    CPB_TRY(grid_ragged(k_poseidon_verify_paths_ragged<F, T>, smem, n, grid));
+    k_poseidon_verify_paths_ragged<F, T><<<grid, kBlock, smem, st>>>(leaf->dev, leaf->d_consts, node->dev, node->d_consts, root, values,
+                                                                     vbase, offsets, siblings, paths, plen, indexes, ok, (long)n);
     CPB_CUDA(cudaGetLastError());
     return CPB_OK;
 }
@@ -387,6 +479,14 @@ cpb_status merkle_build_streams(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, 
     template cpb_status launch_permute_ft<F, T>(cpb_poseidon_ctx*, const u32*, u32*, size_t, cudaStream_t);             \
     template cpb_status launch_verify_ft<F, T>(cpb_poseidon_ctx*, cpb_poseidon_ctx*, const u32*, const u32*, size_t, const u32*, \
                                                const u32*, int, const unsigned long long*, unsigned char*, size_t, cudaStream_t);
+// the ragged kernels live in translation units of their own (poseidon_ragged_<field>.cu), so adding them leaves the code of the
+// uniform kernels exactly as it was
+#define CPB_POS_INSTANTIATE_RAGGED(F, T)                                                                                 \
+    template cpb_status launch_crh_ragged_ft<F, T>(cpb_poseidon_ctx*, const u32*, u64, const u64*, const unsigned*, const unsigned*, \
+                                                   u32*, size_t, size_t, bool, cudaStream_t);                            \
+    template cpb_status launch_verify_ragged_ft<F, T>(cpb_poseidon_ctx*, cpb_poseidon_ctx*, const u32*, const u32*, u64, const u64*, \
+                                                      const u32*, const u32*, int, const unsigned long long*, unsigned char*, size_t, \
+                                                      cudaStream_t);
 #define CPB_POS_INSTANTIATE_TEAM(F) template cpb_status launch_tree_top_f<F>(cpb_poseidon_ctx*, TopJob, cudaStream_t);
 #define CPB_POS_EXTERN_TEAM(F) extern template cpb_status launch_tree_top_f<F>(cpb_poseidon_ctx*, TopJob, cudaStream_t);
 #define CPB_POS_EXTERN(F, T)                                                                                             \
@@ -394,5 +494,11 @@ cpb_status merkle_build_streams(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, 
     extern template cpb_status launch_permute_ft<F, T>(cpb_poseidon_ctx*, const u32*, u32*, size_t, cudaStream_t);      \
     extern template cpb_status launch_verify_ft<F, T>(cpb_poseidon_ctx*, cpb_poseidon_ctx*, const u32*, const u32*, size_t, const u32*, \
                                                       const u32*, int, const unsigned long long*, unsigned char*, size_t, cudaStream_t);
+#define CPB_POS_EXTERN_RAGGED(F, T)                                                                                      \
+    extern template cpb_status launch_crh_ragged_ft<F, T>(cpb_poseidon_ctx*, const u32*, u64, const u64*, const unsigned*,       \
+                                                          const unsigned*, u32*, size_t, size_t, bool, cudaStream_t);           \
+    extern template cpb_status launch_verify_ragged_ft<F, T>(cpb_poseidon_ctx*, cpb_poseidon_ctx*, const u32*, const u32*, u64,  \
+                                                             const u64*, const u32*, const u32*, int, const unsigned long long*, \
+                                                             unsigned char*, size_t, cudaStream_t);
 
 }  // namespace cpb

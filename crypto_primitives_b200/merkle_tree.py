@@ -18,12 +18,19 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _native as N
+from . import ragged as R
 from .crh import pedersen as pedersen_crh
 from .crh import poseidon as poseidon_crh
 
 
 def _p(a):
     return a.ctypes.data_as(N.u64p)
+
+
+def _leaf_batch(leaves):
+    """Leaves as one array -- or, for leaves of different lengths, which no array holds, the sequence itself: the field-leaf
+    Config's leaf hash takes it as a ragged batch (each leaf hashed at its own length, as MerkleTree::new does)."""
+    return leaves if R.is_ragged(leaves) else np.asarray(leaves)
 
 
 class Config:
@@ -77,13 +84,25 @@ class PoseidonFieldConfig(Config):
         return poseidon_crh.TwoToOneCRH.compress_batch(param, pairs, device)
 
     def build(self, leaf_param, two_to_one_param, leaves, device):
+        if R.is_ragged(leaves):
+            return self.build_ragged(leaf_param, two_to_one_param, *R.pack(leaves), device)
         lv = np.ascontiguousarray(leaves, dtype=np.uint64)
-        assert lv.ndim == 3 and lv.shape[2] == 4, "leaves must be (n, leaf_len, 4)"
+        assert lv.ndim == 3 and lv.shape[2] == 4, "leaves must be (n, leaf_len, 4) or a list of (leaf_len_i, 4)"
         n, ln = lv.shape[0], lv.shape[1]
         leaf_nodes = np.empty((n, 4), dtype=np.uint64)
         non_leaf = np.empty((max(n - 1, 0), 4), dtype=np.uint64)
         N.check(N.lib.cpb_merkle_poseidon_build(leaf_param.context(device), two_to_one_param.context(device),
                                                 _p(lv), ln, n, _p(leaf_nodes), _p(non_leaf)))
+        return leaf_nodes, non_leaf
+
+    def build_ragged(self, leaf_param, two_to_one_param, values, offsets, device):
+        """MerkleTree::new over leaves of different lengths: leaf i = values[offsets[i] .. offsets[i+1])."""
+        vals, off = R.as_arrays(values, offsets)
+        n = off.shape[0] - 1
+        leaf_nodes = np.empty((max(n, 0), 4), dtype=np.uint64)
+        non_leaf = np.empty((max(n - 1, 0), 4), dtype=np.uint64)
+        R.check(N.lib.cpb_merkle_poseidon_build_ragged(leaf_param.context(device), two_to_one_param.context(device), _p(vals), _p(off), n,
+                                                       _p(leaf_nodes), _p(non_leaf)))
         return leaf_nodes, non_leaf
 
     def build_from_digests(self, two_to_one_param, leaf_digests, device):
@@ -229,7 +248,7 @@ def verify_paths_batch(leaf_hash_params, two_to_one_params, root_hash, leaves, p
         return np.zeros(0, dtype=bool)
     plen = len(proofs[0].auth_path)
     assert all(len(p.auth_path) == plen for p in proofs), "paths of different heights"
-    claimed = cfg.leaf_hash_batch(leaf_hash_params, np.asarray(leaves), device)
+    claimed = cfg.leaf_hash_batch(leaf_hash_params, _leaf_batch(leaves), device)
     idx = np.array([p.leaf_index for p in proofs], dtype=np.int64)
     cur = _select_and_hash(cfg, two_to_one_params, claimed, np.stack([p.leaf_sibling_hash for p in proofs]), idx & 1, device)
     idx >>= 1
@@ -289,7 +308,7 @@ class MultiPath:
             paths.append(auth)
             prev = auth
         idx = np.array(self.leaf_indexes, dtype=np.int64)
-        claimed = cfg.leaf_hash_batch(leaf_hash_params, np.asarray(leaves), device)
+        claimed = cfg.leaf_hash_batch(leaf_hash_params, _leaf_batch(leaves), device)
         # Level-synchronous form of the reference's loop with its look-up table of already hashed nodes (mod.rs:272-322):
         # at every level each tree node is hashed ONCE, from the first path (in order) that reaches it -- exactly the
         # `hash_lut.entry(..).or_insert_with(..)` semantics -- and all distinct nodes of a level are one device batch.
@@ -412,15 +431,20 @@ class MerkleTree:
         One GPU thread recomputes one root."""
         if not isinstance(self.config, PoseidonFieldConfig):
             raise NotImplementedError("the one-launch kernel is for the Poseidon field-leaf Config; use verify_paths_batch")
-        lv = np.ascontiguousarray(leaves, dtype=np.uint64)
+        if R.is_ragged(leaves):                # leaves of different lengths: (values, offsets)
+            lv, n_leaves = R.pack(leaves), len(leaves)
+        else:
+            lv = np.ascontiguousarray(leaves, dtype=np.uint64)
+            assert lv.ndim == 3
+            n_leaves = lv.shape[0]
         plen = self._height - 2
         if isinstance(proofs, tuple):
             sib, paths, idx = (np.ascontiguousarray(a, dtype=np.uint64) for a in proofs)
             n = idx.shape[0]
-            assert lv.shape[0] == n and lv.ndim == 3 and paths.shape == (n, plen, 4)
+            assert n_leaves == n and paths.shape == (n, plen, 4)
             return self._verify_arrays(lv, sib, paths, idx, root_hash)
         n = len(proofs)
-        assert lv.shape[0] == n and lv.ndim == 3
+        assert n_leaves == n
         sib = np.ascontiguousarray(np.stack([p.leaf_sibling_hash for p in proofs]), dtype=np.uint64)
         paths = np.ascontiguousarray(np.stack([np.stack(p.auth_path) if plen else np.zeros((0, 4), dtype=np.uint64) for p in proofs]),
                                      dtype=np.uint64).reshape(n, plen, 4)
@@ -431,8 +455,13 @@ class MerkleTree:
         n, plen = idx.shape[0], self._height - 2
         root = np.ascontiguousarray(self.root() if root_hash is None else root_hash, dtype=np.uint64)
         ok = np.zeros(n, dtype=np.uint8)
-        N.check(N.lib.cpb_merkle_poseidon_verify_batch(self.leaf_hash_param.context(self.device), self.two_to_one_hash_param.context(self.device),
-                                                       _p(root), _p(lv), lv.shape[1], _p(sib), _p(paths), plen, _p(idx),
+        lctx, nctx = self.leaf_hash_param.context(self.device), self.two_to_one_hash_param.context(self.device)
+        if isinstance(lv, tuple):
+            vals, off = lv
+            R.check(N.lib.cpb_merkle_poseidon_verify_ragged_batch(lctx, nctx, _p(root), _p(vals), _p(off), _p(sib), _p(paths), plen, _p(idx),
+                                                                  ok.ctypes.data_as(N.u8p), n))
+            return ok.astype(bool)
+        N.check(N.lib.cpb_merkle_poseidon_verify_batch(lctx, nctx, _p(root), _p(lv), lv.shape[1], _p(sib), _p(paths), plen, _p(idx),
                                                        ok.ctypes.data_as(N.u8p), n))
         return ok.astype(bool)
 
@@ -445,7 +474,7 @@ class MerkleTree:
         n = self.leaf_nodes.shape[0]
         assert idx.size and idx.min() >= 0 and idx.max() < n, "index out of range"
         assert np.unique(idx).size == idx.size, "indexes must be distinct"
-        new_hash = np.asarray(cfg.leaf_hash_batch(self.leaf_hash_param, np.asarray(new_leaves), dev))
+        new_hash = np.asarray(cfg.leaf_hash_batch(self.leaf_hash_param, _leaf_batch(new_leaves), dev))
         par = np.unique(idx >> 1)                                  # touched leaf pairs
         pairs = np.stack([self.leaf_nodes[2 * par], self.leaf_nodes[2 * par + 1]], axis=1)     # gathers only the touched rows
         pairs[np.searchsorted(par, idx >> 1), idx & 1] = new_hash                              # ... with the new digests patched in

@@ -275,11 +275,27 @@ class PoseidonSponge:
 
 def absorb_squeeze_batch(parameters: PoseidonConfig, inputs, num_squeeze: int, device: int = 0) -> np.ndarray:
     """n independent sponges in one kernel launch: new -> absorb(inputs[i]) -> squeeze_native_field_elements(num_squeeze).
-    inputs (n, len, 4) -> (n, num_squeeze, 4)."""
+    inputs (n, len, 4) -> (n, num_squeeze, 4).  A list of (L_i, 4) arrays whose lengths differ goes through absorb_squeeze_ragged."""
+    from .. import ragged as R
+    if R.is_ragged(inputs):
+        return absorb_squeeze_ragged(parameters, *R.pack(inputs), num_squeeze, device)
     inp = np.ascontiguousarray(inputs, dtype=np.uint64)
     assert inp.ndim == 3 and inp.shape[2] == 4
     n, ln = inp.shape[0], inp.shape[1]
     out = np.empty((n, num_squeeze, 4), dtype=np.uint64)
     N.check(N.lib.cpb_poseidon_sponge_batch(parameters.context(device), inp.ctypes.data_as(N.u64p), ln, out.ctypes.data_as(N.u64p),
                                             num_squeeze, n))
+    return out
+
+
+def absorb_squeeze_ragged(parameters: PoseidonConfig, values, offsets, num_squeeze: int, device: int = 0) -> np.ndarray:
+    """absorb_squeeze_batch over inputs of different lengths: sponge i absorbs values[offsets[i] .. offsets[i+1]).
+    -> (n, num_squeeze, 4) with n = len(offsets) - 1; offsets that decrease raise ValueError."""
+    from .. import ragged as R
+    vals, off = R.as_arrays(values, offsets)
+    n = off.shape[0] - 1
+    out = np.empty((n, num_squeeze, 4), dtype=np.uint64)
+    if n and num_squeeze:
+        R.check(N.lib.cpb_poseidon_sponge_ragged_batch(parameters.context(device), vals.ctypes.data_as(N.u64p), off.ctypes.data_as(N.u64p),
+                                                       out.ctypes.data_as(N.u64p), num_squeeze, n))
     return out

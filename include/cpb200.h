@@ -76,8 +76,8 @@ typedef struct cpb_multi cpb_multi;         /* a group of GPUs driven by one pro
 
 const char* cpb_last_error(void);
 
-/* ABI revision of this header: bumped when entry points or status codes are added (2 = CPB_INTERNAL_ERROR, cpb_abi_version; 3 = _dev field conversion, host pinning, launch count, multi-GPU build, CPB_NCCL_ERROR, wire formats). */
-#define CPB_ABI_VERSION 3
+/* ABI revision of this header: bumped when entry points or status codes are added (2 = CPB_INTERNAL_ERROR, cpb_abi_version; 3 = _dev field conversion, host pinning, launch count, multi-GPU build, CPB_NCCL_ERROR, wire formats; 4 = ragged Poseidon batches: CRH, sponge, Merkle build and path verification over inputs of different lengths). */
+#define CPB_ABI_VERSION 4
 int cpb_abi_version(void);
 int cpb_version(void);
 /* Number of visible CUDA devices with compute capability 10.x (0 when none / no driver). */
@@ -178,6 +178,41 @@ cpb_status cpb_merkle_poseidon_verify_batch_dev(cpb_poseidon_ctx* leaf_ctx, cpb_
                                                 const uint64_t* leaves, size_t leaf_len, const uint64_t* leaf_sibling_hashes,
                                                 const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes,
                                                 uint8_t* ok, size_t n, void* stream);
+
+/* ---- Poseidon over inputs of different lengths (ragged batches) --------------------------------------------------- */
+/* The reference's Poseidon input and field leaf are unsized slices (CRHScheme::Input = [F], R/crh/poseidon/mod.rs:19-41;
+ * Config::Leaf = [F], R/merkle_tree/tests/mod.rs:198-206).  A ragged batch is `values`, field elements back to back, and
+ * `offsets`, n + 1 uint64_t: input i is values[offsets[i] .. offsets[i+1]) (element indices; offsets[0] need not be 0) --
+ * one prefix sum over a Vec<Vec<F>>.  Zero-padding to a common length is not equivalent (absorbing zeros that start a new
+ * rate block adds a permutation), so each input is hashed at its own length.
+ * Host forms: offsets must not decrease (else CPB_BAD_LENGTH); only values[offsets[0] .. offsets[n]) is copied.
+ * _dev forms: offsets (device memory) must not decrease; this is not checked, but a decreasing pair hashes as an empty input
+ * and nothing outside values[offsets[0] .. offsets[n]) is read.  n >= 2^32 -> CPB_BAD_LENGTH; n == 0 -> CPB_OK, no launch.
+ * The device sorts the inputs by permutation count before hashing (stream-ordered scratch, no host synchronisation). */
+cpb_status cpb_poseidon_crh_ragged_batch(cpb_poseidon_ctx* ctx, const uint64_t* values, const uint64_t* offsets, uint64_t* out, size_t n);
+cpb_status cpb_poseidon_crh_ragged_batch_dev(cpb_poseidon_ctx* ctx, const uint64_t* values, const uint64_t* offsets, uint64_t* out,
+                                             size_t n, void* stream);
+/* n sponges: absorb input i, squeeze n_squeeze native elements to out[i * n_squeeze ..]. */
+cpb_status cpb_poseidon_sponge_ragged_batch(cpb_poseidon_ctx* ctx, const uint64_t* values, const uint64_t* offsets, uint64_t* out,
+                                            size_t n_squeeze, size_t n);
+cpb_status cpb_poseidon_sponge_ragged_batch_dev(cpb_poseidon_ctx* ctx, const uint64_t* values, const uint64_t* offsets, uint64_t* out,
+                                                size_t n_squeeze, size_t n, void* stream);
+/* MerkleTree::new over leaves of different lengths (mod.rs:411-422 hashes each leaf at its own length): the ragged leaf hash,
+ * then the inner levels as cpb_merkle_poseidon_from_digests.  Outputs and rules as cpb_merkle_poseidon_build. */
+cpb_status cpb_merkle_poseidon_build_ragged(cpb_poseidon_ctx* leaf_ctx, cpb_poseidon_ctx* node_ctx, const uint64_t* values,
+                                            const uint64_t* offsets, size_t n, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes);
+cpb_status cpb_merkle_poseidon_build_ragged_dev(cpb_poseidon_ctx* leaf_ctx, cpb_poseidon_ctx* node_ctx, const uint64_t* values,
+                                                const uint64_t* offsets, size_t n, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes,
+                                                void* stream);
+/* cpb_merkle_poseidon_verify_batch with leaf i = values[offsets[i] .. offsets[i+1]). */
+cpb_status cpb_merkle_poseidon_verify_ragged_batch(cpb_poseidon_ctx* leaf_ctx, cpb_poseidon_ctx* node_ctx, const uint64_t* root,
+                                                   const uint64_t* values, const uint64_t* offsets, const uint64_t* leaf_sibling_hashes,
+                                                   const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes, uint8_t* ok,
+                                                   size_t n);
+cpb_status cpb_merkle_poseidon_verify_ragged_batch_dev(cpb_poseidon_ctx* leaf_ctx, cpb_poseidon_ctx* node_ctx, const uint64_t* root,
+                                                       const uint64_t* values, const uint64_t* offsets, const uint64_t* leaf_sibling_hashes,
+                                                       const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes,
+                                                       uint8_t* ok, size_t n, void* stream);
 
 /* ---- Pedersen CRH / commitment over a twisted-Edwards curve -------------------------------- */
 /* pedersen::Parameters{generators: Vec<Vec<C>>} (R/crh/pedersen/mod.rs:28-31) and, when n_rand > 0,

@@ -31,6 +31,21 @@ inline void check(cpb_status s) {
     if (s != CPB_OK) throw Error(s, std::string("cpb status ") + std::to_string((int)s) + ": " + cpb_last_error());
 }
 
+// Inputs of different lengths (Vec<Vec<F>>) as the C-ABI's ragged batch: the elements back to back plus n + 1 offsets.
+inline void ragged_pack(const std::vector<std::vector<Fe>>& inputs, std::vector<Fe>& values, std::vector<uint64_t>& offsets) {
+    offsets.assign(1, 0);
+    values.clear();
+    for (const auto& x : inputs) {
+        values.insert(values.end(), x.begin(), x.end());
+        offsets.push_back(values.size());
+    }
+}
+inline bool equal_lengths(const std::vector<std::vector<Fe>>& inputs) {
+    for (const auto& x : inputs)
+        if (x.size() != inputs[0].size()) return false;
+    return true;
+}
+
 namespace poseidon {
 
 // PoseidonConfig<F> (R/sponge/poseidon/mod.rs:26-45) + the device context built from it.
@@ -84,6 +99,19 @@ struct CRH {
         const size_t n = len ? inputs.size() / len : 0;
         std::vector<Fe> out(n);
         if (n) check(cpb_poseidon_crh_batch(p.ctx(), inputs[0].data(), len, out[0].data(), n));
+        return out;
+    }
+    // n inputs of any lengths, each hashed at its own length (one ragged call; equal lengths take the uniform call)
+    static std::vector<Fe> evaluate_batch(const Parameters& p, const std::vector<std::vector<Fe>>& inputs) {
+        std::vector<Fe> out(inputs.size());
+        if (inputs.empty()) return out;
+        std::vector<Fe> values;
+        std::vector<uint64_t> offsets;
+        ragged_pack(inputs, values, offsets);
+        if (equal_lengths(inputs) && !inputs[0].empty())
+            check(cpb_poseidon_crh_batch(p.ctx(), values[0].data(), inputs[0].size(), out[0].data(), out.size()));
+        else
+            check(cpb_poseidon_crh_ragged_batch(p.ctx(), values.empty() ? nullptr : values[0].data(), offsets.data(), out[0].data(), out.size()));
         return out;
     }
 };
@@ -171,6 +199,20 @@ public:
                                         n ? t.leaf_nodes[0].data() : nullptr, n > 1 ? t.non_leaf_nodes[0].data() : nullptr));
         return t;
     }
+    // leaves of different lengths (Config::Leaf = [F]): each leaf hashed at its own length
+    static PoseidonMerkleTree create(const poseidon::Config& leaf, const poseidon::Config& two_to_one, const std::vector<std::vector<Fe>>& leaves) {
+        std::vector<Fe> values;
+        std::vector<uint64_t> offsets;
+        ragged_pack(leaves, values, offsets);
+        if (!leaves.empty() && equal_lengths(leaves) && !leaves[0].empty()) return create(leaf, two_to_one, values, leaves[0].size());
+        PoseidonMerkleTree t;
+        const size_t n = leaves.size();
+        t.leaf_nodes.resize(n);
+        t.non_leaf_nodes.resize(n ? n - 1 : 0);
+        check(cpb_merkle_poseidon_build_ragged(leaf.ctx(), two_to_one.ctx(), values.empty() ? nullptr : values[0].data(), offsets.data(), n,
+                                               n ? t.leaf_nodes[0].data() : nullptr, n > 1 ? t.non_leaf_nodes[0].data() : nullptr));
+        return t;
+    }
     Fe root() const { return non_leaf_nodes.at(0); }
     size_t height() const {
         size_t h = 1, n = leaf_nodes.size();
@@ -194,19 +236,44 @@ public:
     std::vector<uint8_t> verify_batch(const poseidon::Config& leaf, const poseidon::Config& two_to_one, const Fe& root,
                                       const std::vector<size_t>& indexes, const std::vector<Fe>& leaves, size_t leaf_len) const {
         const size_t n = indexes.size(), plen = height() - 2;
-        std::vector<Fe> sib(n), paths(n * plen);
-        std::vector<uint64_t> idx(n);
+        std::vector<Fe> sib, paths;
+        std::vector<uint64_t> idx;
+        proofs(indexes, sib, paths, idx);
+        std::vector<uint8_t> ok(n, 0);
+        if (n)
+            check(cpb_merkle_poseidon_verify_batch(leaf.ctx(), two_to_one.ctx(), root.data(), leaves[0].data(), leaf_len, sib[0].data(),
+                                                   plen ? paths[0].data() : nullptr, plen, idx.data(), ok.data(), n));
+        return ok;
+    }
+    // the same with claimed leaves of different lengths: leaves[i] belongs to indexes[i]
+    std::vector<uint8_t> verify_batch(const poseidon::Config& leaf, const poseidon::Config& two_to_one, const Fe& root,
+                                      const std::vector<size_t>& indexes, const std::vector<std::vector<Fe>>& leaves) const {
+        const size_t n = indexes.size(), plen = height() - 2;
+        if (leaves.size() != n) throw Error(CPB_BAD_LENGTH, "one leaf per index");
+        std::vector<Fe> sib, paths, values;
+        std::vector<uint64_t> idx, offsets;
+        proofs(indexes, sib, paths, idx);
+        ragged_pack(leaves, values, offsets);
+        std::vector<uint8_t> ok(n, 0);
+        if (n)
+            check(cpb_merkle_poseidon_verify_ragged_batch(leaf.ctx(), two_to_one.ctx(), root.data(), values.empty() ? nullptr : values[0].data(),
+                                                          offsets.data(), sib[0].data(), plen ? paths[0].data() : nullptr, plen, idx.data(),
+                                                          ok.data(), n));
+        return ok;
+    }
+
+private:
+    void proofs(const std::vector<size_t>& indexes, std::vector<Fe>& sib, std::vector<Fe>& paths, std::vector<uint64_t>& idx) const {
+        const size_t n = indexes.size(), plen = height() - 2;
+        sib.resize(n);
+        paths.resize(n * plen);
+        idx.resize(n);
         for (size_t i = 0; i < n; i++) {
             sib[i] = leaf_sibling_hash(indexes[i]);
             std::vector<Fe> ap = auth_path(indexes[i]);
             for (size_t k = 0; k < plen; k++) paths[i * plen + k] = ap[k];
             idx[i] = indexes[i];
         }
-        std::vector<uint8_t> ok(n, 0);
-        if (n)
-            check(cpb_merkle_poseidon_verify_batch(leaf.ctx(), two_to_one.ctx(), root.data(), leaves[0].data(), leaf_len, sib[0].data(),
-                                                   plen ? paths[0].data() : nullptr, plen, idx.data(), ok.data(), n));
-        return ok;
     }
 };
 

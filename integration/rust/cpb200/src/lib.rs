@@ -27,6 +27,10 @@ extern "C" {
     fn cpb_poseidon_compress_batch(ctx: *mut cpb_poseidon_ctx, pairs: *const u64, out: *mut u64, n: usize) -> c_int;
     fn cpb_merkle_poseidon_build(leaf: *mut cpb_poseidon_ctx, node: *mut cpb_poseidon_ctx, leaves: *const u64, leaf_len: usize,
                                  n: usize, leaf_nodes: *mut u64, non_leaf_nodes: *mut u64) -> c_int;
+    // inputs of different lengths (ABI v4): input i = values[offsets[i] .. offsets[i+1])
+    fn cpb_poseidon_crh_ragged_batch(ctx: *mut cpb_poseidon_ctx, values: *const u64, offsets: *const u64, out: *mut u64, n: usize) -> c_int;
+    fn cpb_merkle_poseidon_build_ragged(leaf: *mut cpb_poseidon_ctx, node: *mut cpb_poseidon_ctx, values: *const u64, offsets: *const u64,
+                                        n: usize, leaf_nodes: *mut u64, non_leaf_nodes: *mut u64) -> c_int;
     // page-lock a `Vec<Fr>`'s storage once so the host-pointer calls copy at full PCIe rate (ABI v3)
     fn cpb_host_register(ptr: *mut core::ffi::c_void, bytes: usize) -> c_int;
     fn cpb_host_unregister(ptr: *mut core::ffi::c_void) -> c_int;
@@ -95,6 +99,20 @@ gpu_field!(ark_ed_on_bls12_381::FrConfig, 2);
 
 fn flatten<F: GpuField>(xs: &[F]) -> Vec<u64> { xs.iter().flat_map(|x| x.mont_limbs()).collect() }
 fn unflatten<F: GpuField>(l: &[u64]) -> Vec<F> { l.chunks_exact(4).map(|c| F::from_mont_limbs([c[0], c[1], c[2], c[3]])).collect() }
+/// `Some(len)` when every input has the same length (the uniform calls), `None` when they differ (the ragged calls).
+fn common_len<T: AsRef<[F]>, F>(inputs: &[T]) -> Option<usize> {
+    let len = inputs.first().map_or(0, |i| i.as_ref().len());
+    inputs.iter().all(|i| i.as_ref().len() == len).then_some(len)
+}
+/// The ragged layout of the ABI: the inputs' elements back to back and the n + 1 prefix sums of their lengths.
+fn offsets<T: AsRef<[F]>, F>(inputs: &[T]) -> Vec<u64> {
+    let mut off = Vec::with_capacity(inputs.len() + 1);
+    off.push(0u64);
+    for i in inputs {
+        off.push(off[off.len() - 1] + i.as_ref().len() as u64);
+    }
+    off
+}
 
 struct Ctx(*mut cpb_poseidon_ctx);
 unsafe impl Send for Ctx {}
@@ -125,13 +143,18 @@ impl<F: GpuField> GpuPoseidonParams<F> {
 /// `crh::poseidon::CRH` (R/crh/poseidon/mod.rs:15-41) on the GPU.
 pub struct GpuPoseidonCRH<F>(PhantomData<F>);
 impl<F: GpuField> GpuPoseidonCRH<F> {
-    /// n inputs of equal length, one kernel launch.
+    /// n inputs, one call: equal lengths take the uniform kernel, different lengths the ragged call (each input hashed at
+    /// its own length, as `CRH::evaluate` does).
     pub fn evaluate_batch(p: &GpuPoseidonParams<F>, inputs: &[&[F]]) -> Result<Vec<F>, Error> {
-        let len = inputs.first().map_or(0, |i| i.len());
-        assert!(inputs.iter().all(|i| i.len() == len), "batched inputs must have equal length");
         let flat: Vec<u64> = inputs.iter().flat_map(|i| flatten(i)).collect();
         let mut out = vec![0u64; 4 * inputs.len()];
-        check(unsafe { cpb_poseidon_crh_batch(p.ctx.0, flat.as_ptr(), len, out.as_mut_ptr(), inputs.len()) })?;
+        match common_len::<_, F>(inputs) {
+            Some(len) => check(unsafe { cpb_poseidon_crh_batch(p.ctx.0, flat.as_ptr(), len, out.as_mut_ptr(), inputs.len()) })?,
+            None => {
+                let off = offsets::<_, F>(inputs);
+                check(unsafe { cpb_poseidon_crh_ragged_batch(p.ctx.0, flat.as_ptr(), off.as_ptr(), out.as_mut_ptr(), inputs.len()) })?
+            },
+        }
         Ok(unflatten(&out))
     }
 }
@@ -175,13 +198,22 @@ pub struct GpuMerkleTree<F: GpuField> {
     height: usize,
 }
 impl<F: GpuField> GpuMerkleTree<F> {
+    /// `MerkleTree::new` hashes each leaf at its own length (R/merkle_tree/mod.rs:411-422): leaves of different lengths take
+    /// the ragged build, equal lengths the uniform one.
     pub fn new(leaf: &GpuPoseidonParams<F>, two_to_one: &GpuPoseidonParams<F>, leaves: &[Vec<F>]) -> Result<Self, Error> {
         let n = leaves.len();
-        let leaf_len = leaves.first().map_or(0, |l| l.len());
         let flat: Vec<u64> = leaves.iter().flat_map(|l| flatten(l)).collect();
         let (mut ln, mut nn) = (vec![0u64; 4 * n], vec![0u64; 4 * n.saturating_sub(1)]);
         check(unsafe {
-            cpb_merkle_poseidon_build(leaf.ctx.0, two_to_one.ctx.0, flat.as_ptr(), leaf_len, n, ln.as_mut_ptr(), nn.as_mut_ptr())
+            match common_len::<_, F>(leaves) {
+                Some(leaf_len) => cpb_merkle_poseidon_build(leaf.ctx.0, two_to_one.ctx.0, flat.as_ptr(), leaf_len, n, ln.as_mut_ptr(),
+                                                            nn.as_mut_ptr()),
+                None => {
+                    let off = offsets::<_, F>(leaves);
+                    cpb_merkle_poseidon_build_ragged(leaf.ctx.0, two_to_one.ctx.0, flat.as_ptr(), off.as_ptr(), n, ln.as_mut_ptr(),
+                                                     nn.as_mut_ptr())
+                },
+            }
         })?;
         Ok(Self { leaf_nodes: unflatten(&ln), non_leaf_nodes: unflatten(&nn), height: n.trailing_zeros() as usize + 1 })
     }
@@ -221,7 +253,8 @@ impl GpuGroup {
         -> Result<GpuMerkleTree<F>, Error> {
         assert!(leaf.len() == self.ndev && two_to_one.len() == self.ndev, "one context per device");
         let n = leaves.len();
-        let leaf_len = leaves.first().map_or(0, |l| l.len());
+        // the sharded build takes one leaf length; leaves of different lengths would be hashed wrongly, so refuse them
+        let leaf_len = common_len::<_, F>(leaves).expect("the multi-GPU build needs leaves of equal length; use GpuMerkleTree::new for others");
         let mut flat: Vec<u64> = leaves.iter().flat_map(|l| flatten(l)).collect();
         let (mut ln, mut nn) = (vec![0u64; 4 * n], vec![0u64; 4 * n.saturating_sub(1)]);
         let lc: Vec<*mut cpb_poseidon_ctx> = leaf.iter().map(|p| p.ctx.0).collect();
