@@ -718,10 +718,13 @@ cpb_status cpb_poseidon_ctx_create(int field_id, int rate, int capacity, int ful
     c->sms = sm_count(device);
     c->sched = host::derive_schedule(F, P, true);
     c->dev = to_dev(c->sched);
-    size_t bytes = c->sched.consts.size() * 8;
+    size_t bytes = c->sched.consts.size() * 8, tab_bytes = c->sched.tabs.size() * 8;
     if (bytes > 200 * 1024) { delete c; return fail(CPB_UNSUPPORTED, "round schedule (%zu B) exceeds shared memory", bytes); }
-    cudaError_t e = cudaMalloc(&c->d_consts, bytes);
+    cudaError_t e = cudaMalloc(&c->d_consts, bytes + tab_bytes);      // staged schedule, then the digit tables (global memory)
     if (e == cudaSuccess) e = cudaMemcpy(c->d_consts, c->sched.consts.data(), bytes, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && tab_bytes)
+        e = cudaMemcpy(c->d_consts + bytes / 4, c->sched.tabs.data(), tab_bytes, cudaMemcpyHostToDevice);
+    if (tab_bytes) c->dev.tab = c->d_consts + bytes / 4;
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) {
         if (c->d_consts) cudaFree(c->d_consts);

@@ -515,6 +515,88 @@ template <class F, int T, int XI> CPB_HD void fp_dot_unit(u32* r, const u32 (&a)
     for (int i = 0; i < 8; i++) r[i] = w[i];
 }
 
+// ---------------------------------------------------------------------------------------
+// Dot product with fixed coefficients through digit tables: r = sum_{j<T} a[j] * c_j (+ y) mod p with TWO reduction rows.
+// The coefficient c_j (Montgomery form) is known ahead of time, so instead of reducing each of the 8 rows of a[j] * c_j the
+// host pre-reduces its digit multiples K_i(c_j) = c_j * 2^(32 i) * 2^64 / R mod p (i = 0..7, canonical plain integers; the
+// schedule's digit tables, poseidon_host.hpp).  Then  V = sum_j sum_i a[j][i] * K_i(c_j) == (sum_j a[j] * c_j / R) * 2^64  and
+// two Montgomery rows divide by 2^64.  The rows are 8T scalar x vector products at the same limb offset (a[j]'s limb is the
+// scalar, the table row the vector): 64T + 16 wide multiply-adds (64T + 12 for BLS12-381 Fr) instead of fp_dot's 64T + 64.
+//   V < 8T * 2^32 * p = T * 2^35 * p, for ANY a[j] < 2^256 (lazy outputs included), plus y * 2^64 for the unit addend (U = 1,
+//   y in [0,p), added at limbs 2..9 with additions only).  The accumulator is E, O (limbs 0..8) and the overflow word X (limb 9).
+//   Result = (V + M*p) / 2^64 with M < 2^64: below p * (1 + U + T * 2^-29), brought to [0,p) by U + 1 conditional subtractions
+//   (2p then p when U = 1: 2 + T * 2^-29 < 4).  With w-bit limbs (the toy-field model) read 2^32, 2^64 as 2^w, 2^2w.
+// tab: T tables of 8 rows of 8 limbs (K_0(c_j) .. K_7(c_j)), read with 128-bit loads.  r must not alias a; it may alias y.
+// ---------------------------------------------------------------------------------------
+namespace detail {
+
+// Overflow word needed by the product rows (without the unit addend): the 8T rows plus a reduction row stay below 2^288 iff
+// (8T + 1) * p <= 2^256 (decided on the top limb, as dot_needs_x).  The unit addend's top limb lands on limb 9 itself.
+template <class F, int T, int U> CPB_HD constexpr bool tab_needs_x() { return U > 0 || dot_needs_x<F, 8 * T>(); }
+
+// Conditional subtractions after the two rows: the smallest K with (1 + U) * 2^29 + T <= 2^(K + 30) (result bound above; the
+// limb width enters as 2^29 = 2^32 / 8).
+template <int T, int U> CPB_HD constexpr int tab_reduce_passes() {
+    int k = 0;
+    while (((long long)(1 + U) << (LIMB_BITS - 3)) + T > ((long long)1 << (k + 1 + LIMB_BITS - 3))) k++;
+    return k;
+}
+
+// A table row is stored odd limbs first (K[1], K[3], K[5], K[7], K[0], K[2], K[4], K[6]): each 128-bit load feeds one of the
+// two carry chains of acc_row_x.
+CPB_HD void ld_tab_row(u32* r, const u32* p) {
+#if defined(__CUDA_ARCH__)
+    const uint4 o = __ldg(reinterpret_cast<const uint4*>(p));
+    const uint4 e = __ldg(reinterpret_cast<const uint4*>(p + 4));
+    r[1] = o.x; r[3] = o.y; r[5] = o.z; r[7] = o.w;
+    r[0] = e.x; r[2] = e.y; r[4] = e.z; r[6] = e.w;
+#else
+    for (int i = 0; i < 4; i++) {
+        r[2 * i + 1] = p[i];
+        r[2 * i] = p[4 + i];
+    }
+#endif
+}
+
+}  // namespace detail
+
+template <class F, int T, int U = 0>
+CPB_HD void fp_dot_tab(u32* r, const u32 (*a)[8], const u32* tab, const u32* pm, const u32* y = nullptr) {
+    static_assert(U == 0 || U == 1, "fp_dot_tab takes at most one unit addend");
+    constexpr bool WX = detail::tab_needs_x<F, T, U>();
+    u32 ev[8], od[8], X = 0, k[8];
+    detail::ld_tab_row(k, tab);
+#pragma unroll
+    for (int j = 0; j < 8; j += 2) {
+        mul_wide(ev[j], ev[j + 1], k[j], a[0][0]);
+        mul_wide(od[j], od[j + 1], k[j + 1], a[0][0]);
+    }
+#pragma unroll
+    for (int q = 1; q < 8 * T; q++) {
+        detail::ld_tab_row(k, tab + 8 * q);                    // K_i(c_j), q = 8j + i
+        detail::acc_row_x<WX>(ev, od, X, k, a[q / 8][q % 8]);
+    }
+    if (U) {                                                   // + y * 2^64: limbs 2..7 in ev, 8 in od[7], 9 in X
+        ev[2] = add_cc(ev[2], y[0]);
+#pragma unroll
+        for (int i = 3; i < 8; i++) ev[i] = addc_cc(ev[i], y[i - 2]);
+        od[7] = addc_cc(od[7], y[6]);
+        X = addc(X, y[7]);
+    }
+    detail::redc_row_x<F>(ev, od, X, pm);
+    detail::redc_row_shift_x<F>(od, ev, X, 0u, pm);
+    // as fp_dot: the last row used E = od (low limb zero), O = ev
+    u32 w[9];
+    w[0] = add_cc(ev[0], od[1]);
+#pragma unroll
+    for (int i = 1; i < 7; i++) w[i] = addc_cc(ev[i], od[i + 1]);
+    w[7] = addc_cc(ev[7], 0);
+    w[8] = addc(X, 0);
+    detail::reduce9<F, detail::tab_reduce_passes<T, U>()>(w);
+#pragma unroll
+    for (int i = 0; i < 8; i++) r[i] = w[i];
+}
+
 // r = a + b mod p, fully reduced, for a < 2p (an output of the LAZY multiplier) and b in [0,p): a + b < 3p, brought to [0,p)
 // by two conditional subtractions, 2p then p.  Needs 3p < 2^256 (the F::LAZY5 fields).  r may alias a or b.
 template <class F> CPB_HD void fp_add_lazy(u32* r, const u32* a, const u32* b) {

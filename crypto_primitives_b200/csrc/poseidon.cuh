@@ -21,7 +21,34 @@ struct PoseidonDev {
     // warp-uniform address are promoted to uniform registers, and a multiply-add with a
     // uniform-register factor is emitted as IMAD.X + IMAD.HI.U32.X instead of one IMAD.WIDE.U32.X.
     int zero;
+    // Digit tables of the sparse schedule (PoseidonSchedule::tabs) in global memory: pos_permute_split multiplies by its
+    // constants through them (fp_dot_tab).  Every device context has them; a CPU build of this code driven without them
+    // (nullptr) multiplies by the Montgomery rows of `cs` instead, as the merged loop and the team kernel always do.
+    const u32* tab = nullptr;
 };
+
+// This thread's pointer to P.tab.  On the device it is offset by threadIdx.x * zero for the reason given at `zero`.
+CPB_HD const u32* pos_tables(const PoseidonDev& P) {
+#if defined(__CUDA_ARCH__)
+    return P.tab + (int)threadIdx.x * P.zero;
+#else
+    return P.tab;
+#endif
+}
+// Whether pos_permute_split takes the table path: always on the device (the fallback is not compiled there).
+CPB_HD bool pos_has_tables(const PoseidonDev& P) {
+#if defined(__CUDA_ARCH__)
+    return true;
+#else
+    return P.tab != nullptr;
+#endif
+}
+// Element offsets (x 8 limbs) of the digit tables of the full-round matrix of round fr, of the per-round partial constants and
+// of the entry row (PoseidonSchedule::tabs): M, Mpre, Mpost, then the off_sc0 + 1 region; 8 elements per constant.
+CPB_HD int pos_full_table(const PoseidonDev& P, int fr) {
+    const int half = P.rf / 2;
+    return 8 * P.t * P.t * (fr == half - 1 ? 1 : fr == half ? 2 : 0);
+}
 
 template <class F, int T> CPB_HD void pos_add_vec(u32 (&s)[T][8], const u32* c) {
 #pragma unroll
@@ -120,9 +147,12 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
     // put lane 1 into that basis on entry.
     const u32* lp = cs + 8 * (P.off_sc0 + 1);
     const u32* lp_entry = lp + 8 * P.rp * (2 * T - 2);
-    u32 n[T][8];
-#pragma unroll
-    for (int i = 0; i < T; i++) fp_zero(n[i]);
+    // Digit tables (fp_dot_tab): every product by a schedule constant below goes through them -- two reduction rows per output
+    // instead of eight -- and takes any operand below 2^256, so the lazy lanes need no EX term.  tk: the lp region's tables.
+    const bool tabs = pos_has_tables(P);
+    const u32* tb = pos_tables(P);
+    const u32* tk = tb + 64 * 3 * T * T;
+    const u32* tk_entry = tk + 64 * P.rp * (2 * T - 2);
 #pragma unroll 1
     for (int phase = 0; phase < 2; phase++) {
         const int cnt = phase == 0 ? half : P.rf - half;   // odd RF: floor(RF/2) rounds before, ceil(RF/2) after (mod.rs:98-121)
@@ -139,12 +169,21 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
                 pos_rotl<T>(s);
             }
             const u32* rows = cs + 8 * pos_full_matrix(P, phase * half + q);
+            const u32* trows = tb + 8 * pos_full_table(P, phase * half + q);
             const bool entry = phase == 0 && q == cnt - 1;                                 // Mpre: row 1 of the split form
+            // Row collector, zeroed per round so that it is dead in the partial-round loop (24 registers at t = 3, which the
+            // table rows of fp_dot_tab need there) and the shift below never reads an indeterminate value.
+            u32 n[T][8];
+#pragma unroll
+            for (int i = 0; i < T; i++) fp_zero(n[i]);
 #pragma unroll 1
             for (int i = 0; i < T; i++) {
                 u32 d[8];
                 fp_zero(d);
-                if ((need >> i) & 1u) fp_dot<F, T, LZ ? 1 : 0>(d, s, (entry && i == 1) ? lp_entry : rows + 8 * T * i, pm);
+                if ((need >> i) & 1u) {
+                    if (tabs) fp_dot_tab<F, T>(d, s, (entry && i == 1) ? tk_entry : trows + 64 * T * i, pm);
+                    else fp_dot<F, T, LZ ? 1 : 0>(d, s, (entry && i == 1) ? lp_entry : rows + 8 * T * i, pm);
+                }
 #pragma unroll
                 for (int k = 0; k + 1 < T; k++) fp_copy(n[k], n[k + 1]);
                 fp_copy(n[T - 1], d);
@@ -169,8 +208,11 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
             // takes it as its one unreduced term (EX = 1) and returns a canonical a'; d = y + a < 2.60p is made canonical by two
             // conditional subtractions (fp_add_lazy); the column products v_j * y are ordinary multiplications whose full operand
             // y + p stays below 2^256 and whose results are reduced, so lanes 2.. stay canonical.  Bit-identical outputs.
+            // With the digit tables the dot takes y like any operand below 2^256, and the column update s_j' = s_j + v_j * y is one
+            // fp_dot_tab term with the canonical s_j as its unit addend: result canonical (fp.cuh), so lanes 2.. stay canonical.
+            const u32* trow = tk;
 #pragma unroll 1
-            for (int k = 0; k < P.rp; k++, row += 8 * (2 * T - 2), pc += 8) {
+            for (int k = 0; k < P.rp; k++, row += 8 * (2 * T - 2), trow += 64 * (2 * T - 2), pc += 8) {
 #if CPB_SBOX5
                 if (P.alpha == 5) {                   // straight-line x^5
                     u32 x2[8];
@@ -182,13 +224,19 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
                 if (alpha_zero) fp_one<F>(s[0]);
                 else pos_sbox<F>(s[0], P.alpha, top_bit, pm);
                 u32 an[8];
-                fp_dot<F, T, LZ ? 1 : 0>(an, s, row, pm);                // row = [gamma, alpha, beta[2..T-1]]
+                if (tabs) fp_dot_tab<F, T>(an, s, trow, pm);             // row = [gamma, alpha, beta[2..T-1]]
+                else fp_dot<F, T, LZ ? 1 : 0>(an, s, row, pm);
                 if constexpr (LZ) fp_add_lazy<F>(s[1], s[0], s[1]);      // s[1] <- d = y + a
                 else fp_add<F>(s[1], s[0], s[1]);
                 const u32* v = row + 8 * T;                               // v[2..T-1]
+                const u32* tv = trow + 64 * T;
                 if (T <= CPB_COL_UNROLL_MAX) {
 #pragma unroll
                     for (int j = 2; j < T; j++) {
+                        if (tabs) {
+                            fp_dot_tab<F, 1, 1>(s[j], &s[0], tv + 64 * (j - 2), pm, s[j]);
+                            continue;
+                        }
                         u32 c[8], tmp[8];
                         ld_elem(c, v + 8 * (j - 2));
                         fp_mul<F>(tmp, s[0], c, pm);
@@ -198,9 +246,13 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
 #pragma unroll 1
                     for (int j = 2; j < T; j++) {
                         u32 c[8], tmp[8];
-                        ld_elem(c, v + 8 * (j - 2));
-                        fp_mul<F>(tmp, s[0], c, pm);
-                        fp_add<F>(s[2], s[2], tmp);
+                        if (tabs) {
+                            fp_dot_tab<F, 1, 1>(s[2], &s[0], tv + 64 * (j - 2), pm, s[2]);
+                        } else {
+                            ld_elem(c, v + 8 * (j - 2));
+                            fp_mul<F>(tmp, s[0], c, pm);
+                            fp_add<F>(s[2], s[2], tmp);
+                        }
                         fp_copy(tmp, s[2]);                               // rotate lanes 2..T-1
 #pragma unroll
                         for (int q = 2; q + 1 < T; q++) fp_copy(s[q], s[q + 1]);

@@ -138,7 +138,27 @@ struct PoseidonSchedule {
                        //          Mpre's row 1 (t) and Cp0's entry 1 for lane 1 carried as w_hat . s (pos_permute_split only)
     int n_elems = 0;
     std::vector<u64> consts;
+    // Digit tables of fp_dot_tab (sparse only; empty when dense), placed right after the n_elems staged elements of the device
+    // buffer and read from global memory: 8 elements K_0(c) .. K_7(c) per constant c that pos_permute_split multiplies by, for
+    // M, Mpre, Mpost (t x t each, row-major) and then the off_sc0 + 1 region up to (not including) Cp0's entry 1.
+    std::vector<u64> tabs;
 };
+
+// The elements K_i(c) = c * 2^(32 i) * 2^64 mod p (c plain, i.e. c_mont * 2^(32 i + 64) / R) fp_dot_tab multiplies the limbs of
+// its variable operand by, each stored as the 32-bit limbs 1, 3, 5, 7, 0, 2, 4, 6 (detail::ld_tab_row, fp.cuh).
+inline void push_digit_table(const Field& F, const Fe& c, std::vector<u64>& out) {
+    Fe z{{0, 1, 0, 0}};                                   // 2^64 < p
+    for (int i = 0; i < 8; i++) {
+        const Fe k = F.mul(c, z);                         // c_mont * z / R
+        u64 w[4];
+        for (int j = 0; j < 2; j++) {
+            w[j] = (k.l[2 * j] >> 32) | (k.l[2 * j + 1] & 0xffffffff00000000ull);       // limbs 4j+1, 4j+3
+            w[2 + j] = (k.l[2 * j] & 0xffffffffull) | (k.l[2 * j + 1] << 32);          // limbs 4j, 4j+2
+        }
+        out.insert(out.end(), w, w + 4);
+        for (int b = 0; b < 32; b++) z = F.add(z, z);
+    }
+}
 
 namespace detail {
 inline FeVec matmul(const Field& F, const FeVec& A, const FeVec& B, int n) {
@@ -352,6 +372,12 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
     }
     push(lp);                      // at off_sc0 + 1 (pos_permute_split); empty when dense
     S.n_elems = (int)(S.consts.size() / 4);
+    if (sparse) {
+        const FeVec* mats[3] = {&M, &Mpre, &Mpost};
+        for (const FeVec* m : mats)
+            for (const Fe& c : *m) push_digit_table(F, c, S.tabs);
+        for (size_t i = 0; i + 1 < lp.size(); i++) push_digit_table(F, lp[i], S.tabs);
+    }
     return S;
 }
 
