@@ -314,9 +314,6 @@ template <class F> CPB_HD void redc_row_x(u32* E, u32* O, u32& X, const u32* pm)
 // window at 2^256.  The two-limb shift of the old even accumulator is folded into the addend operand of the odd
 // chain's multiply-adds (as next_row does for a product row), so it costs no instructions.
 // tin + X may carry (X = 1 is common, tin = 0xffffffff a 2^-32 event): both are added with carry-out into the new X.
-#ifndef CPB_SQR_FOLD
-#define CPB_SQR_FOLD 1
-#endif
 template <class F> CPB_HD void redc_row_shift_x(u32* E, u32* O, u32& X, u32 tin, const u32* pm) {
     E[0] = add_cc(E[0], O[1]);
     u32 xn;
@@ -358,6 +355,44 @@ template <class F> CPB_HD void redc_row_shift_x(u32* E, u32* O, u32& X, u32 tin,
     }
     O[7] = addc_cc(O[7], 0u);
     X = addc(xn, 0u);
+}
+
+// The same row without an overflow word, for a window that provably stays below 2^288 (fp_sqr, the second row of fp_dot_tab):
+// t7 and t8 enter at 2^224 and 2^256 after the shift, through the addend of the odd chain's top multiply-add, and the chains end
+// without a carry out.
+template <class F> CPB_HD void redc_row_shift(u32* E, u32* O, u32 t7, u32 t8, const u32* pm) {
+    E[0] = add_cc(E[0], O[1]);
+    if (F::P0_ONE) {
+        const u32 c0 = addc(0u, 0u);                  // carry into 2^32; joins the even chain below
+        const u32 e0 = E[0];
+        const u32 m = sub_cc(0u, e0);                 // CF = (e0 != 0)
+        if (F::P1_ALLONES) {
+            const u32 hi1 = subc(m, 0u);              // m - [m != 0]
+            O[0] = add_cc(O[2], e0);
+            O[1] = addc_cc(O[3], hi1);
+        } else {
+            mad_wide_cc_from(O[0], O[1], pm[1], m, O[2], O[3]);
+        }
+        madc_wide_cc_from(O[2], O[3], pm[3], m, O[4], O[5]);
+        madc_wide_cc_from(O[4], O[5], pm[5], m, O[6], O[7]);
+        madc_wide_end_from(O[6], O[7], pm[7], m, t7, t8);
+        (void)add_cc(e0, LIMB_MASK);                  // CF = (e0 != 0): the carry out of E[0] + m
+        E[1] = addc_cc(E[1], c0);
+        madc_wide_cc(E[2], E[3], pm[2], m);
+        madc_wide_cc(E[4], E[5], pm[4], m);
+        madc_wide_cc(E[6], E[7], pm[6], m);
+    } else {
+        const u32 m = mul_lo(E[0], F::NINV);          // (does not touch the carry flag)
+        madc_wide_cc_from(O[0], O[1], pm[1], m, O[2], O[3]);
+        madc_wide_cc_from(O[2], O[3], pm[3], m, O[4], O[5]);
+        madc_wide_cc_from(O[4], O[5], pm[5], m, O[6], O[7]);
+        madc_wide_end_from(O[6], O[7], pm[7], m, t7, t8);
+        mad_wide_cc(E[0], E[1], pm[0], m);
+        madc_wide_cc(E[2], E[3], pm[2], m);
+        madc_wide_cc(E[4], E[5], pm[4], m);
+        madc_wide_cc(E[6], E[7], pm[6], m);
+    }
+    O[7] = addc(O[7], 0u);
 }
 
 // V += a * bi   (no shift).  WX: keep the overflow word X up to date (see fp_dot for when it is needed).
@@ -405,19 +440,22 @@ template <class F> CPB_HD constexpr u32 p_shl(int k, int i) {
                   ((i > 0 && k > 0) ? ((u64)F::P(i - 1) >> (LIMB_BITS - k)) : 0ull)) & LIMB_MASK);
 }
 
-// r (9 limbs) < 2^(K+1) * p  ->  r[0..7] in [0,p)
-template <class F, int K> CPB_HD void reduce9(u32* r) {
+// r (N = 9 limbs) < 2^(K+1) * p  ->  r[0..7] in [0, 2^KLO * p): conditional subtractions of 2^K p, ..., 2^KLO p.  N = 8: r < 2^256.
+template <class F, int K, int KLO = 0, int N = 9> CPB_HD void reduce9(u32* r) {
+    static_assert(N == 9 || N == 8, "9 limbs, or 8 for a value below 2^256");
+    static_assert(N == 9 || p_shl<F>(K, 8) == 0, "2^K p must fit 8 limbs");
 #pragma unroll
-    for (int k = K; k >= 0; k--) {
-        u32 t[9];
+    for (int k = K; k >= KLO; k--) {
+        u32 t[N];
         t[0] = sub_cc(r[0], p_shl<F>(k, 0));
 #pragma unroll
-        for (int i = 1; i < 9; i++) t[i] = subc_cc(r[i], p_shl<F>(k, i));
+        for (int i = 1; i < N; i++) t[i] = subc_cc(r[i], p_shl<F>(k, i));
         u32 borrow = subc(0, 0);
 #pragma unroll
-        for (int i = 0; i < 9; i++) r[i] = borrow ? r[i] : t[i];
+        for (int i = 0; i < N; i++) r[i] = borrow ? r[i] : t[i];
     }
 }
+template <class F, int K, int KLO = 0> CPB_HD void reduce8(u32* r) { reduce9<F, K, KLO, 8>(r); }
 
 // The running value of a T-term dot product stays below (T+1) * p * 2^32.  When (T+1) * p <= 2^256 that fits the 9 limbs
 // of (E, O) and the overflow word is dead weight: 5 ALU instructions per row.  Decided on the top limb (p < (p[7]+1) * 2^224):
@@ -522,10 +560,12 @@ template <class F, int T, int XI> CPB_HD void fp_dot_unit(u32* r, const u32 (&a)
 // schedule's digit tables, poseidon_host.hpp).  Then  V = sum_j sum_i a[j][i] * K_i(c_j) == (sum_j a[j] * c_j / R) * 2^64  and
 // two Montgomery rows divide by 2^64.  The rows are 8T scalar x vector products at the same limb offset (a[j]'s limb is the
 // scalar, the table row the vector): 64T + 16 wide multiply-adds (64T + 12 for BLS12-381 Fr) instead of fp_dot's 64T + 64.
-//   V < 8T * 2^32 * p = T * 2^35 * p, for ANY a[j] < 2^256 (lazy outputs included), plus y * 2^64 for the unit addend (U = 1,
-//   y in [0,p), added at limbs 2..9 with additions only).  The accumulator is E, O (limbs 0..8) and the overflow word X (limb 9).
-//   Result = (V + M*p) / 2^64 with M < 2^64: below p * (1 + U + T * 2^-29), brought to [0,p) by U + 1 conditional subtractions
-//   (2p then p when U = 1: 2 + T * 2^-29 < 4).  With w-bit limbs (the toy-field model) read 2^32, 2^64 as 2^w, 2^2w.
+//   V < 8T * 2^32 * p = T * 2^35 * p, for ANY a[j] < 2^256 (lazy outputs included), plus y * 2^64 for the unit addend (U > 0,
+//   y in [0, U*p), added at limbs 2..9 with additions only).  The accumulator is E, O (limbs 0..8) and the overflow word X (limb 9);
+//   U = 2 needs the slack tab_fits checks.
+//   Result = (V + M*p) / 2^64 with M < 2^64: below p * (1 + U + T * 2^-29), brought to [0,p) by conditional subtractions of
+//   2^K p, ..., p (K = 1 for U = 1, 2: below 4p).  LAZY: the last one, by p, is skipped and the result left in [0, 2p) -- below
+//   p * (1 + T * 2^-29) when U = 0.  With w-bit limbs (the toy-field model) read 2^32, 2^64 as 2^w, 2^2w.
 // tab: T tables of 8 rows of 8 limbs (K_0(c_j) .. K_7(c_j)), read with 128-bit loads.  r must not alias a; it may alias y.
 // ---------------------------------------------------------------------------------------
 namespace detail {
@@ -533,6 +573,21 @@ namespace detail {
 // Overflow word needed by the product rows (without the unit addend): the 8T rows plus a reduction row stay below 2^288 iff
 // (8T + 1) * p <= 2^256 (decided on the top limb, as dot_needs_x).  The unit addend's top limb lands on limb 9 itself.
 template <class F, int T, int U> CPB_HD constexpr bool tab_needs_x() { return U > 0 || dot_needs_x<F, 8 * T>(); }
+
+// The accumulator's ten limbs (E, O, X) hold V + M*p < p * (8T * 2^32 + (1 + U) * 2^64) iff
+// (p[7] + 1) * (1 + U + 8T * 2^-32) <= 2^32 (on the top limb): a unit addend below 2p (U = 2) needs about 3p < 2^256 -- every
+// field tag but BLS12-381 Fr.
+template <class F, int T, int U> CPB_HD constexpr bool tab_fits() {
+    return ((u64)F::P(7) + 1) * (1 + U) + ((((u64)F::P(7) + 1) * 8 * T + LIMB_MASK) >> LIMB_BITS) <= ((u64)1 << LIMB_BITS);
+}
+
+// Overflow word of the second reduction row: after it (before the final shift) the value is (V + m0*p)/2^32 + m1*p, below
+// p * (8T + 1 + (1 + U) * 2^32).  That stays below 2^288 -- so X is dead in the second row -- when
+// (p[7] + 1) * (8T + 1 + (1 + U) * 2^32) <= 2^64 (on the top limb, p < (p[7] + 1) * 2^224), and the result is then below 2^256.
+// BN254 Fr for U <= 2, BLS12-381 Fr for U <= 1.
+template <class F, int T, int U> CPB_HD constexpr bool tab_row2_needs_x() {
+    return ((u64)F::P(7) + 1) * (1 + U) + ((((u64)F::P(7) + 1) * (8 * T + 1) + LIMB_MASK) >> LIMB_BITS) > ((u64)1 << LIMB_BITS);
+}
 
 // Conditional subtractions after the two rows: the smallest K with (1 + U) * 2^29 + T <= 2^(K + 30) (result bound above; the
 // limb width enters as 2^29 = 2^32 / 8).
@@ -560,9 +615,10 @@ CPB_HD void ld_tab_row(u32* r, const u32* p) {
 
 }  // namespace detail
 
-template <class F, int T, int U = 0>
+template <class F, int T, int U = 0, bool LAZY = false>
 CPB_HD void fp_dot_tab(u32* r, const u32 (*a)[8], const u32* tab, const u32* pm, const u32* y = nullptr) {
-    static_assert(U == 0 || U == 1, "fp_dot_tab takes at most one unit addend");
+    static_assert(U >= 0 && U <= 2, "fp_dot_tab takes one unit addend below 2p at most");
+    static_assert(U < 2 || detail::tab_fits<F, T, U>(), "the accumulator does not hold a unit addend below 2p");
     constexpr bool WX = detail::tab_needs_x<F, T, U>();
     u32 ev[8], od[8], X = 0, k[8];
     detail::ld_tab_row(k, tab);
@@ -583,22 +639,37 @@ CPB_HD void fp_dot_tab(u32* r, const u32 (*a)[8], const u32* tab, const u32* pm,
         od[7] = addc_cc(od[7], y[6]);
         X = addc(X, y[7]);
     }
-    detail::redc_row_x<F>(ev, od, X, pm);
-    detail::redc_row_shift_x<F>(od, ev, X, 0u, pm);
+    constexpr int K = detail::tab_reduce_passes<T, U>(), KLO = LAZY ? 1 : 0;
+    if (WX) detail::redc_row_x<F>(ev, od, X, pm);
+    else detail::redc_row<F>(ev, od, pm);
     // as fp_dot: the last row used E = od (low limb zero), O = ev
-    u32 w[9];
-    w[0] = add_cc(ev[0], od[1]);
+    if constexpr (detail::tab_row2_needs_x<F, T, U>()) {
+        detail::redc_row_shift_x<F>(od, ev, X, 0u, pm);
+        u32 w[9];
+        w[0] = add_cc(ev[0], od[1]);
 #pragma unroll
-    for (int i = 1; i < 7; i++) w[i] = addc_cc(ev[i], od[i + 1]);
-    w[7] = addc_cc(ev[7], 0);
-    w[8] = addc(X, 0);
-    detail::reduce9<F, detail::tab_reduce_passes<T, U>()>(w);
+        for (int i = 1; i < 7; i++) w[i] = addc_cc(ev[i], od[i + 1]);
+        w[7] = addc_cc(ev[7], 0);
+        w[8] = addc(X, 0);
+        detail::reduce9<F, K, KLO>(w);
 #pragma unroll
-    for (int i = 0; i < 8; i++) r[i] = w[i];
+        for (int i = 0; i < 8; i++) r[i] = w[i];
+    } else {                                                   // result < 2^256: 8 limbs
+        detail::redc_row_shift<F>(od, ev, 0u, WX ? X : 0u, pm);
+        u32 w[8];
+        w[0] = add_cc(ev[0], od[1]);
+#pragma unroll
+        for (int i = 1; i < 7; i++) w[i] = addc_cc(ev[i], od[i + 1]);
+        w[7] = addc(ev[7], 0);
+        detail::reduce8<F, K, KLO>(w);
+#pragma unroll
+        for (int i = 0; i < 8; i++) r[i] = w[i];
+    }
 }
 
-// r = a + b mod p, fully reduced, for a < 2p (an output of the LAZY multiplier) and b in [0,p): a + b < 3p, brought to [0,p)
-// by two conditional subtractions, 2p then p.  Needs 3p < 2^256 (the F::LAZY5 fields).  r may alias a or b.
+// r = a + b mod p, fully reduced, for a + b < 3p (a < 2p an output of the LAZY multiplier, b in [0,p) or slightly above, as a
+// LAZY fp_dot_tab leaves it): brought to [0,p) by two conditional subtractions, 2p then p.  Needs 3p < 2^256 (the F::LAZY5
+// fields).  r may alias a or b.
 template <class F> CPB_HD void fp_add_lazy(u32* r, const u32* a, const u32* b) {
     static_assert(3 * ((u64)F::P(7) + 1) <= ((u64)1 << LIMB_BITS), "fp_add_lazy needs 3p < 2^256");
     fp_add_noreduce(r, a, b);
@@ -681,43 +752,30 @@ template <class F, bool LAZY> CPB_HD void fp_sqr(u32* r, const u32* a, const u32
     mad_wide_cc(T[0], T[1], a[0], a[0]);
 #pragma unroll
     for (int i = 1; i < 8; i++) madc_wide_cc(T[2 * i], T[2 * i + 1], a[i], a[i]);
-    // Montgomery reduction of the 16-limb T with a rolling 9-limb window (ev, od) + overflow word X
-    u32 ev[8], od[8], X = 0;
+    // Montgomery reduction of the 16-limb T with a rolling 9-limb window (ev, od) and no overflow word.  Limb i + 7 of T enters at
+    // row i (i >= 1), limb 15 after the last row, so after row i the window holds (T mod 2^(32(i+8)) + M*p) / 2^(32i) with
+    // M < 2^(32(i+1)): below 2^256 + 2^32*p < 2^288 for ANY a < 2^256 whenever p < 2^256 - 2^224 (every field tag).  The
+    // result (T + M*p)/R is the same value the per-row entry at 2^256 computes.
+    static_assert(F::P(7) < LIMB_MASK, "fp_sqr's window bound needs p < 2^256 - 2^224");
+    u32 ev[8], od[8];
 #pragma unroll
     for (int i = 0; i < 8; i++) { ev[i] = T[i]; od[i] = 0; }
-    od[7] = T[8];
-    detail::redc_row_x<F>(ev, od, X, pm);
+    detail::redc_row<F>(ev, od, pm);
 #pragma unroll
     for (int i = 1; i < 8; i++) {
         // shift the window by one limb: roles of ev/od swap each row
         u32* Ea = (i & 1) ? od : ev;    // new even accumulator (previous odd)
         u32* Oa = (i & 1) ? ev : od;    // previous even accumulator: low limb is zero, limb 1 moves into Ea[0]
-#if CPB_SQR_FOLD
-        detail::redc_row_shift_x<F>(Ea, Oa, X, T[(i + 8) & 15], pm);
-        continue;
-#endif
-        Ea[0] = add_cc(Ea[0], Oa[1]);
-#pragma unroll
-        for (int k = 0; k < 6; k++) Oa[k] = addc_cc(Oa[k + 2], 0);
-        Oa[6] = addc_cc(0, 0);
-        // the previous row's overflow word meets the next limb of T here; their sum can carry
-        // (X = 1 is common, T[i + 8] = 0xffffffff is a 2^-32 event -- or an adversarial input)
-        Oa[7] = addc_cc((i + 8 < 16) ? T[i + 8] : 0u, X);
-        X = addc(0, 0);
-        detail::redc_row_x<F>(Ea, Oa, X, pm);
+        detail::redc_row_shift<F>(Ea, Oa, T[i + 7], 0u, pm);
     }
-    // 8 rows: the last used E = od (low limb zero), O = ev
-    u32 w[9];
+    // 8 rows: the last used E = od (low limb zero), O = ev; T[15] lands on limb 7.  The result is below 2p < 2^256 (a < p, or
+    // a^2 < R*p when LAZY), so nothing carries out of limb 7.
+    u32 w[8];
     w[0] = add_cc(ev[0], od[1]);
 #pragma unroll
     for (int i = 1; i < 7; i++) w[i] = addc_cc(ev[i], od[i + 1]);
-    if (LAZY) {                        // result < 2p < 2^256: limb 8 is zero
-        w[7] = addc(ev[7], 0);
-    } else {
-        w[7] = addc_cc(ev[7], 0);
-        w[8] = addc(X, 0);
-        detail::reduce9<F, 0>(w);      // T < p^2  =>  result < 2p
-    }
+    w[7] = addc(ev[7], T[15]);
+    if (!LAZY) fp_final_sub<F>(w);     // T < p^2  =>  result < 2p
 #pragma unroll
     for (int i = 0; i < 8; i++) r[i] = w[i];
 }

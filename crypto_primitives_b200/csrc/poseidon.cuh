@@ -97,6 +97,15 @@ template <class F> CPB_HD void pos_sbox(u32* x, u64 alpha, int top_bit, const u3
     }
 }
 
+// x^5 as sqr, sqr, mul.  LAZY (F::LAZY5 fields): the three products skip their conditional subtractions (bounds at pos_sbox and
+// pos_permute_split).
+template <class F, bool LAZY> CPB_HD void pos_sbox5(u32* x, const u32* pm) {
+    u32 x2[8];
+    fp_sqr<F, LAZY>(x2, x, pm);
+    fp_sqr<F, LAZY>(x2, x2, pm);
+    fp_mul<F, LAZY>(x, x2, x, pm);
+}
+
 // The permutation, one rolled loop over all RF+RP rounds with a single instance of each
 // arithmetic body:  [add round constants] -> S-box on T lanes or lane 0 -> linear layer as
 // lazy dot products (T rows of a dense matrix, or the one dense row of the sparse form
@@ -130,18 +139,22 @@ struct PermuteHint {
     unsigned need;         // bit i set: lane i of the result is read; everything else is dead
 };
 
-template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* cs, const u32* pm, const PermuteHint& H) {
+// A5: the exponent is 5, known at compile time (P.alpha is not read).  Every S-box is then the straight-line pos_sbox5, with no
+// run-time exponent test and no generic square-and-multiply body in either loop.
+template <class F, int T, bool A5 = false>
+CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* cs, const u32* pm, const PermuteHint& H) {
     const int half = P.rf / 2;
     int top_bit = 0;
-    for (int i = 63; i > 0; i--)
-        if ((P.alpha >> i) & 1) { top_bit = i; break; }
-    const bool alpha_zero = P.alpha == 0;
+    if (!A5)
+        for (int i = 63; i > 0; i--)
+            if ((P.alpha >> i) & 1) { top_bit = i; break; }
+    const bool alpha_zero = !A5 && P.alpha == 0;
     // Lazy reduction (F::LAZY5: p/2^256 <= 0.19, i.e. BN254 Fr; alpha = 5; widths whose (T+1)-term rows need no overflow word).
     // Full rounds: the S-box of a canonical x skips its three conditional subtractions (x^5 < 1.24p, see pos_sbox) and the dense
     // rows take the T unreduced lanes as EX = 1 (T * 1.24p < (T+1)*p for T <= 4), returning canonical values.
     constexpr bool LZ = F::LAZY5 && !detail::dot_needs_x<F, T + 1>() && T <= 4;
     static_assert(!F::LAZY5 || 100 * ((u64)F::P(7) + 1) <= 19 * ((u64)1 << LIMB_BITS), "LAZY5 needs p/2^256 <= 0.19");
-    const bool lazy = LZ && CPB_SBOX5 && P.alpha == 5;
+    const bool lazy = LZ && (A5 || (CPB_SBOX5 && P.alpha == 5));
     // Lane 1 is carried as a = w_hat . s through the partial rounds (poseidon_host.hpp).  Its coefficients follow S(c0) in the
     // schedule (so PoseidonDev needs no field): per round [gamma, alpha, beta | v[2..T-1]], then the Mpre row and Cp0 entry that
     // put lane 1 into that basis on entry.
@@ -164,6 +177,7 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
 #pragma unroll 1
             for (int j = 0; j < T; j++) {
                 if (j == first_j) ld_elem(s[0], cs + 8 * P.off_sc0);         // S(0 + c) of the schedule
+                else if constexpr (A5) pos_sbox5<F, LZ>(s[0], pm);
                 else if (alpha_zero) fp_one<F>(s[0]);
                 else pos_sbox<F>(s[0], P.alpha, top_bit, pm, lazy);
                 pos_rotl<T>(s);
@@ -209,22 +223,32 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
             // conditional subtractions (fp_add_lazy); the column products v_j * y are ordinary multiplications whose full operand
             // y + p stays below 2^256 and whose results are reduced, so lanes 2.. stay canonical.  Bit-identical outputs.
             // With the digit tables the dot takes y like any operand below 2^256, and the column update s_j' = s_j + v_j * y is one
-            // fp_dot_tab term with the canonical s_j as its unit addend: result canonical (fp.cuh), so lanes 2.. stay canonical.
+            // fp_dot_tab term with s_j as its unit addend.
+            // Wide lanes (table path; every bound in tests/test_poseidon_bn254_alu.py).  The tables take any operand below 2^256, so
+            // lanes 1.. need not be canonical inside the loop; only the additions that follow them and the exit care:
+            //   lanes j >= 2 in [0, 2p) (WC: fields whose accumulator holds a unit addend below 2p, tab_fits -- not BLS12-381 Fr): the
+            //     column update takes s_j < 2p as its unit addend (U = 2, result < p*(3 + 2^-29)) and one conditional subtraction of
+            //     2p brings it back below 2p (the pass by p is skipped).
+            //   lane 1 (LZ only): a' = the dot's result below p*(1 + T*2^-29) with its one conditional subtraction skipped.  Its one
+            //     addition is d = y + a' < 1.60p + 1.01p < 3p, which fp_add_lazy brings to [0, p) as before.
+            // After the last round lanes 1.. are made canonical (one pass by p), so the second-half constant additions see [0, p).
+            constexpr bool WC = detail::tab_fits<F, 1, 2>();
+            constexpr int UC = WC ? 2 : 1;
             const u32* trow = tk;
 #pragma unroll 1
             for (int k = 0; k < P.rp; k++, row += 8 * (2 * T - 2), trow += 64 * (2 * T - 2), pc += 8) {
+                if constexpr (A5) {
+                    pos_sbox5<F, LZ>(s[0], pm);
+                } else {
 #if CPB_SBOX5
-                if (P.alpha == 5) {                   // straight-line x^5
-                    u32 x2[8];
-                    fp_sqr<F, LZ>(x2, s[0], pm);
-                    fp_sqr<F, LZ>(x2, x2, pm);
-                    fp_mul<F, LZ>(s[0], x2, s[0], pm);
-                } else
+                    if (P.alpha == 5) pos_sbox5<F, LZ>(s[0], pm);     // straight-line x^5
+                    else
 #endif
-                if (alpha_zero) fp_one<F>(s[0]);
-                else pos_sbox<F>(s[0], P.alpha, top_bit, pm);
+                    if (alpha_zero) fp_one<F>(s[0]);
+                    else pos_sbox<F>(s[0], P.alpha, top_bit, pm);
+                }
                 u32 an[8];
-                if (tabs) fp_dot_tab<F, T>(an, s, trow, pm);             // row = [gamma, alpha, beta[2..T-1]]
+                if (tabs) fp_dot_tab<F, T, 0, LZ>(an, s, trow, pm);      // row = [gamma, alpha, beta[2..T-1]]
                 else fp_dot<F, T, LZ ? 1 : 0>(an, s, row, pm);
                 if constexpr (LZ) fp_add_lazy<F>(s[1], s[0], s[1]);      // s[1] <- d = y + a
                 else fp_add<F>(s[1], s[0], s[1]);
@@ -234,7 +258,7 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
 #pragma unroll
                     for (int j = 2; j < T; j++) {
                         if (tabs) {
-                            fp_dot_tab<F, 1, 1>(s[j], &s[0], tv + 64 * (j - 2), pm, s[j]);
+                            fp_dot_tab<F, 1, UC, WC>(s[j], &s[0], tv + 64 * (j - 2), pm, s[j]);
                             continue;
                         }
                         u32 c[8], tmp[8];
@@ -247,7 +271,7 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
                     for (int j = 2; j < T; j++) {
                         u32 c[8], tmp[8];
                         if (tabs) {
-                            fp_dot_tab<F, 1, 1>(s[2], &s[0], tv + 64 * (j - 2), pm, s[2]);
+                            fp_dot_tab<F, 1, UC, WC>(s[2], &s[0], tv + 64 * (j - 2), pm, s[2]);
                         } else {
                             ld_elem(c, v + 8 * (j - 2));
                             fp_mul<F>(tmp, s[0], c, pm);
@@ -269,15 +293,18 @@ template <class F, int T> CPB_HD void pos_permute_split(u32 (&s)[T][8], const Po
                 }
                 fp_copy(s[1], an);
             }
+#pragma unroll
+            for (int i = 1; i < T; i++) fp_final_sub<F>(s[i]);
         }
     }
 }
 
-template <class F, int T> CPB_HD void pos_permute(u32 (&s)[T][8], const PoseidonDev& P, const u32* cs, const u32* pm,
-                                                  const PermuteHint& H = PermuteHint{0, ~0u}) {
+// A5: see pos_permute_split; dense schedules take the merged loop, which reads P.alpha.
+template <class F, int T, bool A5 = false>
+CPB_HD void pos_permute(u32 (&s)[T][8], const PoseidonDev& P, const u32* cs, const u32* pm, const PermuteHint& H = PermuteHint{0, ~0u}) {
     if constexpr (CPB_POS_SPLIT_FOR(F)) {
         if (P.sparse) {
-            pos_permute_split<F, T>(s, P, cs, pm, H);
+            pos_permute_split<F, T, A5>(s, P, cs, pm, H);
             return;
         }
     }
@@ -410,8 +437,8 @@ CPB_HD void pos_sponge(u32* out, long n_out, const u32* in, long len, const Pose
 
 // The one-permutation case of pos_sponge (len <= rate, 1 <= n_out <= rate, capacity >= 1) -- every hash of a Merkle build and
 // every CRH::evaluate / TwoToOneCRH::compress of up to `rate` elements -- with the permutation told what the sponge knows
-// (PermuteHint): lane 0 enters as zero, and only lanes cap .. cap+n_out-1 of the result are read.
-template <class F, int T>
+// (PermuteHint): lane 0 enters as zero, and only lanes cap .. cap+n_out-1 of the result are read.  A5: P.alpha == 5 (pos_permute_split).
+template <class F, int T, bool A5 = false>
 CPB_HD void pos_hash_single(u32* out, int n_out, const u32* in, int len, const PoseidonDev& P, const u32* cs, const u32* pm) {
     u32 s[T][8];
     const int cap = P.cap;
@@ -421,7 +448,7 @@ CPB_HD void pos_hash_single(u32* out, int n_out, const u32* in, int len, const P
         if (lane >= 0 && lane < len) ld_elem(s[i], in + 8 * lane);
         else fp_zero(s[i]);
     }
-    pos_permute<F, T>(s, P, cs, pm, PermuteHint{1, ((1u << n_out) - 1u) << cap});
+    pos_permute<F, T, A5>(s, P, cs, pm, PermuteHint{1, ((1u << n_out) - 1u) << cap});
 #pragma unroll
     for (int i = 0; i < T; i++) {
         const int lane = i - cap;

@@ -19,7 +19,8 @@ constexpr int kBlock = 128;
 constexpr int pos_min_blocks(int t) { return t <= 3 ? CPB_POS_MINB3 : t <= 5 ? 3 : 1; }
 
 // SINGLE: len <= rate, 1 <= n_out <= rate, capacity >= 1 (checked by launch_crh_ft): one permutation per hash, pos_hash_single.
-template <class F, int T, bool SINGLE>
+// A5 (SINGLE only): alpha == 5 compiled in (pos_permute_split); launch_crh_ft picks it where pos_alpha5_kernel says it exists.
+template <class F, int T, bool SINGLE, bool A5 = false>
 __global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
 k_poseidon_crh(PoseidonDev P, const u32* __restrict__ consts, const u32* __restrict__ in, u32* __restrict__ out,
                long n, long len, long n_out) {
@@ -31,10 +32,14 @@ k_poseidon_crh(PoseidonDev P, const u32* __restrict__ consts, const u32* __restr
     ld_elem(pm, ct + 8 * P.off_mod);
     const long stride = (long)gridDim.x * blockDim.x;
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        if constexpr (SINGLE) pos_hash_single<F, T>(out + 8 * n_out * i, (int)n_out, in + 8 * len * i, (int)len, P, ct, pm);
+        if constexpr (SINGLE) pos_hash_single<F, T, A5>(out + 8 * n_out * i, (int)n_out, in + 8 * len * i, (int)len, P, ct, pm);
         else pos_sponge<F, T>(out + 8 * n_out * i, n_out, in + 8 * len * i, len, P, ct, pm);
     }
 }
+
+// The (field, width) pairs with an alpha = 5 one-permutation kernel: BN254 Fr at t = 3, the configuration of the Merkle benchmark
+// (2-element leaves and two-to-one nodes, alpha = 5).  Every other pair, and any other exponent, runs the generic kernel.
+template <class F, int T> constexpr bool pos_alpha5_kernel() { return F::ID == Bn254_Fr::ID && T == 3; }
 
 template <class F, int T>
 __global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
@@ -112,6 +117,14 @@ cpb_status launch_crh_ft(cpb_poseidon_ctx* c, const u32* in, size_t len, u32* ou
     size_t smem = (size_t)c->dev.n_elems * 32;
     int grid = 1;
     const bool single = len <= (size_t)c->dev.rate && n_out >= 1 && n_out <= (size_t)c->dev.rate && c->dev.cap >= 1;
+    if constexpr (pos_alpha5_kernel<F, T>()) {
+        if (single && c->dev.alpha == 5) {
+            CPB_TRY(grid_for(k_poseidon_crh<F, T, true, true>, smem, c->sms, (long)n, grid));
+            k_poseidon_crh<F, T, true, true><<<grid, kBlock, smem, st>>>(c->dev, c->d_consts, in, out, (long)n, (long)len, (long)n_out);
+            CPB_CUDA(cudaGetLastError());
+            return CPB_OK;
+        }
+    }
     if (single) {
         CPB_TRY(grid_for(k_poseidon_crh<F, T, true>, smem, c->sms, (long)n, grid));
         k_poseidon_crh<F, T, true><<<grid, kBlock, smem, st>>>(c->dev, c->d_consts, in, out, (long)n, (long)len, (long)n_out);

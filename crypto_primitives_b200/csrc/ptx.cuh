@@ -70,6 +70,11 @@ CPB_D void madc_wide_end(u32& lo, u32& hi, u32 a, u32 b) {
 CPB_D void madc_wide_end_from(u32& lo, u32& hi, u32 a, u32 b, u32 c_lo) {
     asm volatile("madc.lo.cc.u32 %0, %2, %3, %4; madc.hi.u32 %1, %2, %3, 0;" : "=&r"(lo), "=r"(hi) : "r"(a), "r"(b), "r"(c_lo));
 }
+// (lo,hi) = a*b + (c_lo,c_hi) + CF; ends a chain (callers prove the sum below 2^64).
+CPB_D void madc_wide_end_from(u32& lo, u32& hi, u32 a, u32 b, u32 c_lo, u32 c_hi) {
+    asm volatile("madc.lo.cc.u32 %0, %2, %3, %4; madc.hi.u32 %1, %2, %3, %5;"
+                 : "=&r"(lo), "=r"(hi) : "r"(a), "r"(b), "r"(c_lo), "r"(c_hi));
+}
 // (lo,hi) = a*b + c_lo; no carry in or out.
 CPB_D void mad_wide_end_from(u32& lo, u32& hi, u32 a, u32 b, u32 c_lo) {
     asm volatile("mad.lo.cc.u32 %0, %2, %3, %4; madc.hi.u32 %1, %2, %3, 0;" : "=&r"(lo), "=r"(hi) : "r"(a), "r"(b), "r"(c_lo));
@@ -117,6 +122,10 @@ inline void madc_wide_end(u32& lo, u32& hi, u32 a, u32 b) {
 }
 inline void madc_wide_end_from(u32& lo, u32& hi, u32 a, u32 b, u32 c_lo) {
     unsigned __int128 s = (unsigned __int128)((u64)a * b) + c_lo + detail::cf();
+    detail::split(s, lo, hi);
+}
+inline void madc_wide_end_from(u32& lo, u32& hi, u32 a, u32 b, u32 c_lo, u32 c_hi) {
+    unsigned __int128 s = (unsigned __int128)detail::join(c_lo, c_hi) + (u64)a * b + detail::cf();
     detail::split(s, lo, hi);
 }
 inline void mad_wide_end_from(u32& lo, u32& hi, u32 a, u32 b, u32 c_lo) {
