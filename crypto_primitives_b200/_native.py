@@ -60,6 +60,10 @@ SIGNATURES = {
     "cpb_merkle_poseidon_build_dev": (C.c_int, [vp, vp, vp, C.c_size_t, C.c_size_t, vp, vp, vp]),
     "cpb_merkle_poseidon_from_digests": (C.c_int, [vp, u64p, C.c_size_t, u64p]),
     "cpb_merkle_poseidon_from_digests_dev": (C.c_int, [vp, vp, C.c_size_t, vp, vp]),
+    "cpb_merkle_poseidon_update_digests_dev": (C.c_int, [vp, vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp, vp, vp]),
+    "cpb_merkle_poseidon_update_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, vp, vp, C.c_size_t, C.c_size_t, vp, vp, vp]),
+    "cpb_merkle_poseidon_update_digests": (C.c_int, [vp, u64p, u64p, C.c_size_t, u64p, u64p, C.c_size_t, u64p, C.POINTER(C.c_int)]),
+    "cpb_merkle_poseidon_update": (C.c_int, [vp, vp, u64p, u64p, C.c_size_t, u64p, u64p, C.c_size_t, C.c_size_t, u64p, C.POINTER(C.c_int)]),
     "cpb_pedersen_ctx_create": (C.c_int, [C.c_int, C.c_int, C.c_int, u64p, C.c_size_t, u64p, C.c_int, C.POINTER(vp)]),
     "cpb_pedersen_ctx_create_ex": (C.c_int, [C.c_int, C.c_int, C.c_int, u64p, C.c_size_t, u64p, C.c_int, C.c_int, C.POINTER(vp)]),
     "cpb_pedersen_ctx_destroy": (None, [vp]),

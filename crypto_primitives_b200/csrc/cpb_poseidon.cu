@@ -145,6 +145,9 @@ PoseidonDev to_dev(const host::PoseidonSchedule& S) {
         case CPB_BLS12_377_FR: CPB_FOR_T(Bls12_377_Fr, M, __VA_ARGS__)               \
     }
 
+}  // namespace
+
+namespace cpb {
 // Largest level (in hashes) handled by the four-warp tree-top kernel: beyond ~6000 hashes the GPU's 528 warp
 // schedulers (132 SMs) are all busy with one hash per thread anyway, and the kernel's grid is capped at 128 CTAs of 32 hashes.
 // CPB_TEAM_MAX overrides (0 disables; values above 4096 are clamped).
@@ -168,7 +171,9 @@ size_t team_max_for(size_t S) {
     return v < team_max() ? v : team_max();
 }
 bool team_capable(const cpb_poseidon_ctx* c) { return c->dev.t == 3 && c->dev.cap == 1 && c->dev.alpha >= 2; }
+}  // namespace cpb
 
+namespace {
 cpb_status launch_tree_top(cpb_poseidon_ctx* c, const TopJob& J, cudaStream_t st) {
     switch (c->field_id) {
         case CPB_BLS12_381_FR: return launch_tree_top_f<Bls12_381_Fr>(c, J, st);

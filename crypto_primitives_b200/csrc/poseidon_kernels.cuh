@@ -334,14 +334,23 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
     return t;
 }
 
-// 32 two-to-one hashes by the 128 threads of the CTA: thread (w, lane) -- pair/out are THIS lane's pointers.
+// Leading-bit indexes of alpha and alpha - 1, the exponents of team_phase1.
+__device__ __forceinline__ void team_top_bits(const PoseidonDev& P, int& tb_alpha, int& tb_e) {
+    tb_alpha = 0;
+    tb_e = 0;
+    for (int i = 63; i > 0; i--)
+        if ((P.alpha >> i) & 1) { tb_alpha = i; break; }
+    for (int i = 63; i > 0; i--)
+        if (((P.alpha - 1) >> i) & 1) { tb_e = i; break; }
+}
+
+// The permutation of 32 two-to-one states by the 128 threads of the CTA: thread (w, lane) enters with lane w of its state in s
+// (zero for w = 0 and w = 3) and, for w = 1, leaves with the digest in s.
 template <class F>
-__device__ __forceinline__ void team_compress32(const u32* pair, u32* out, bool active, int w, int lane, const PoseidonDev& P,
-                                                const u32* ct, const u32* pm, u32* xb, int tb_alpha, int tb_e) {
-    u32 s[8], t[8];
+__device__ __forceinline__ void team_permute32(u32* s, int w, int lane, const PoseidonDev& P, const u32* ct, const u32* pm, u32* xb,
+                                               int tb_alpha, int tb_e) {
+    u32 t[8];
     fp_zero(t);
-    if (w == 1 || w == 2) ld_elem_cg(s, pair + 8 * (w - 1));
-    else fp_zero(s);
     const int total = P.rf + P.rp;
 #pragma unroll 1
     for (int r = 0; r < total; r++) {
@@ -351,6 +360,16 @@ __device__ __forceinline__ void team_compress32(const u32* pair, u32* out, bool 
         team_publish<F>(s, w, lane, r, P, ct, xb);
         __syncthreads();
     }
+}
+
+// 32 two-to-one hashes by the 128 threads of the CTA: thread (w, lane) -- pair/out are THIS lane's pointers.
+template <class F>
+__device__ __forceinline__ void team_compress32(const u32* pair, u32* out, bool active, int w, int lane, const PoseidonDev& P,
+                                                const u32* ct, const u32* pm, u32* xb, int tb_alpha, int tb_e) {
+    u32 s[8];
+    if (w == 1 || w == 2) ld_elem_cg(s, pair + 8 * (w - 1));
+    else fp_zero(s);
+    team_permute32<F>(s, w, lane, P, ct, pm, xb, tb_alpha, tb_e);
     if (w == 1 && active) st_elem(out, s);
 }
 
@@ -366,11 +385,8 @@ k_poseidon_tree_top(PoseidonDev P, const u32* __restrict__ consts, TopJob J) {
     const u32* ct = cs + (int)threadIdx.x * P.zero;
     u32 pm[8];
     ld_elem(pm, ct + 8 * P.off_mod);
-    int tb_alpha = 0, tb_e = 0;
-    for (int i = 63; i > 0; i--)
-        if ((P.alpha >> i) & 1) { tb_alpha = i; break; }
-    for (int i = 63; i > 0; i--)
-        if (((P.alpha - 1) >> i) & 1) { tb_e = i; break; }
+    int tb_alpha, tb_e;
+    team_top_bits(P, tb_alpha, tb_e);
 
     const bool flat = J.flat_in != nullptr;
     unsigned done = 0;
@@ -478,6 +494,9 @@ struct MerkleHost {
 };
 cpb_status check_ctx(const cpb_poseidon_ctx* c);
 bool pow2_gt1(size_t n);
+size_t team_max();
+size_t team_max_for(size_t S);
+bool team_capable(const cpb_poseidon_ctx* c);
 cpb_status launch_crh(cpb_poseidon_ctx* c, const u32* in, size_t len, u32* out, size_t n, cudaStream_t st, size_t n_out = 1);
 cpb_status merkle_subtree_levels(cpb_poseidon_ctx* node, const u32* leaf_digests, size_t n, u32* nodes, size_t S, size_t k,
                                  cudaStream_t st, const MerkleHost* H = nullptr, const ExchangeDev* X = nullptr, int* small_from = nullptr);

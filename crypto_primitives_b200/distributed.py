@@ -133,6 +133,34 @@ class CudaPoseidonBackend:
                                                                      self._stream()))
         return nodes
 
+    def _update_args(self, leaf_nodes, nodes, indexes, asserted_root):
+        n = leaf_nodes.shape[0]
+        assert leaf_nodes.is_contiguous() and nodes.is_contiguous() and tuple(nodes.shape) == (n - 1, 4) and leaf_nodes.shape[1] == 4
+        idx = indexes.to(device=leaf_nodes.device, dtype=torch.int64).contiguous()
+        root = None if asserted_root is None else asserted_root.to(device=leaf_nodes.device, dtype=torch.int64).contiguous().clone()
+        applied = torch.empty(1, dtype=torch.uint8, device=leaf_nodes.device)
+        return n, idx, root, applied
+
+    def update(self, leaf_nodes: torch.Tensor, nodes: torch.Tensor, indexes: torch.Tensor, new_leaves: torch.Tensor, asserted_root=None):
+        """k x MerkleTree::update -- or check_update when `asserted_root` (4,) is given -- on a tree built on this device, in place and
+        on the current stream: leaf_nodes (n, 4), nodes (n-1, 4) heap order, indexes (k,) (the last occurrence of a repeated index
+        wins; an index >= n is skipped), new_leaves (k, L, 4).  Returns the device flag `applied` (uint8, (1,)); no synchronisation."""
+        n, idx, root, applied = self._update_args(leaf_nodes, nodes, indexes, asserted_root)
+        lv = new_leaves.contiguous()
+        k, L = lv.shape[0], lv.shape[1] if lv.dim() > 1 else 0
+        assert idx.shape[0] == k, "one new leaf per index"
+        self.N.check(self.N.lib.cpb_merkle_poseidon_update_dev(self.leaf_ctx, self.node_ctx, leaf_nodes.data_ptr(), nodes.data_ptr(), n,
+                                                               idx.data_ptr(), lv.data_ptr(), L, k, None if root is None else root.data_ptr(),
+                                                               applied.data_ptr(), self._stream()))
+        return applied
+
+    def _update_digests(self, leaf_nodes, nodes, idx, digests, root, applied):
+        self.N.check(self.N.lib.cpb_merkle_poseidon_update_digests_dev(self.node_ctx, leaf_nodes.data_ptr(), nodes.data_ptr(), leaf_nodes.shape[0],
+                                                                       idx.data_ptr(), digests.data_ptr(), idx.shape[0],
+                                                                       None if root is None else root.data_ptr(), applied.data_ptr(),
+                                                                       self._stream()))
+        return applied
+
 
 class CudaMixedBackend(CudaPoseidonBackend):
     """BASELINE config 5: byte leaves hashed with PedersenCRHCompressor (x-coordinate, R/crh/injective_map/mod.rs:22-62),
@@ -169,6 +197,18 @@ class CudaMixedBackend(CudaPoseidonBackend):
         self.N.check(self.N.lib.cpb_pedersen_crh_x_batch_dev(self.leaf_ctx, leaves.data_ptr(), ln, leaves.stride(0), out.data_ptr(), n,
                                                              self._stream()))
         return out
+
+    def update(self, leaf_nodes: torch.Tensor, nodes: torch.Tensor, indexes: torch.Tensor, new_leaves: torch.Tensor, asserted_root=None):
+        """CudaPoseidonBackend.update with byte leaves new_leaves (k, leaf_len) uint8: their Pedersen x-coordinate digests go to a
+        workspace of their own (the "leaf" workspace may hold this tree's leaf digests), then the digest form of the update."""
+        n, idx, root, applied = self._update_args(leaf_nodes, nodes, indexes, asserted_root)
+        k, ln = new_leaves.shape
+        assert idx.shape[0] == k, "one new leaf per index"
+        digests = self._buf("update_leaf", (k, 4), leaf_nodes.device)
+        if k:
+            self.N.check(self.N.lib.cpb_pedersen_crh_x_batch_dev(self.leaf_ctx, new_leaves.data_ptr(), ln, new_leaves.stride(0), digests.data_ptr(),
+                                                                 k, self._stream()))
+        return self._update_digests(leaf_nodes, nodes, idx, digests, root, applied)
 
 
 @dataclass

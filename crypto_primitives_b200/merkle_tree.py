@@ -9,10 +9,12 @@ mod.rs:547-623.  Verification and update are LEVEL-SYNCHRONOUS device batches fo
 (or all touched nodes) of one tree level go through ONE two-to-one batch call, so k proofs / k updated
 leaves cost height launches, not k * height (`verify_paths_batch`, `MultiPath.verify`, `update_batch`);
 the Poseidon field-leaf Config additionally has a single-launch kernel that recomputes one root per
-thread (`cpb_merkle_poseidon_verify_batch`).
+thread (`cpb_merkle_poseidon_verify_batch`), and Configs whose inner hash is Poseidon update in ONE library
+call (`cpb_merkle_poseidon_update_digests`: every level on the device, only touched nodes cross PCIe).
 """
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass
 
 import numpy as np
@@ -465,15 +467,40 @@ class MerkleTree:
                                                        ok.ctypes.data_as(N.u8p), n))
         return ok.astype(bool)
 
+    def _check_indexes(self, indexes):
+        idx = np.asarray(indexes, dtype=np.int64).reshape(-1)
+        assert idx.size and idx.min() >= 0 and idx.max() < self.leaf_nodes.shape[0], "index out of range"
+        assert np.unique(idx).size == idx.size, "indexes must be distinct"
+        return idx
+
+    def _updates_on_device(self) -> bool:
+        """Configs whose inner hash is poseidon::TwoToOneCRH update through cpb_merkle_poseidon_update_digests: the touched nodes
+        of every level are hashed on the device in one call, and only they and the siblings they read cross PCIe."""
+        return type(self.config) in (PoseidonFieldConfig, PedersenPoseidonConfig)
+
+    def _update_digests(self, idx, new_leaves, asserted_new_root=None) -> bool:
+        """The Config's leaf hash of `new_leaves`, then one update call on the tree's arrays in place; True when applied."""
+        cfg, dev = self.config, self.device
+        new_hash = np.ascontiguousarray(cfg.leaf_hash_batch(self.leaf_hash_param, _leaf_batch(new_leaves), dev), dtype=np.uint64).reshape(-1, 4)
+        assert new_hash.shape[0] == idx.size, "one new leaf per index"
+        self.leaf_nodes = np.ascontiguousarray(self.leaf_nodes, dtype=np.uint64)
+        self.non_leaf_nodes = np.ascontiguousarray(self.non_leaf_nodes, dtype=np.uint64)
+        ix = np.ascontiguousarray(idx, dtype=np.uint64)
+        root = None if asserted_new_root is None else np.ascontiguousarray(asserted_new_root, dtype=np.uint64).reshape(4)
+        ok = C.c_int(0)
+        N.check(N.lib.cpb_merkle_poseidon_update_digests(self.two_to_one_hash_param.context(dev), _p(self.leaf_nodes), _p(self.non_leaf_nodes),
+                                                         self.leaf_nodes.shape[0], _p(ix), _p(new_hash), ix.size,
+                                                         None if root is None else _p(root), C.byref(ok)))
+        return bool(ok.value)
+
     def _updated_nodes(self, indexes, new_leaves):
         """The nodes that change when leaves `indexes` (distinct) are replaced by `new_leaves` (mod.rs:627-677 for one leaf):
         -> (new leaf digests, [(heap indexes, new values)] bottom level first).  Level-synchronous: the new leaves are one
-        leaf-hash batch and all touched nodes of a level one two-to-one batch -- height launches for any number of leaves."""
+        leaf-hash batch and all touched nodes of a level one two-to-one batch -- height launches for any number of leaves.
+        The path of Configs without a Poseidon inner hash (Pedersen / Bowe-Hopwood nodes, toy Configs)."""
         cfg, dev = self.config, self.device
-        idx = np.asarray(indexes, dtype=np.int64).reshape(-1)
+        idx = self._check_indexes(indexes)
         n = self.leaf_nodes.shape[0]
-        assert idx.size and idx.min() >= 0 and idx.max() < n, "index out of range"
-        assert np.unique(idx).size == idx.size, "indexes must be distinct"
         new_hash = np.asarray(cfg.leaf_hash_batch(self.leaf_hash_param, _leaf_batch(new_leaves), dev))
         par = np.unique(idx >> 1)                                  # touched leaf pairs
         pairs = np.stack([self.leaf_nodes[2 * par], self.leaf_nodes[2 * par + 1]], axis=1)     # gathers only the touched rows
@@ -498,6 +525,9 @@ class MerkleTree:
     def update_batch(self, indexes, new_leaves):
         """k x MerkleTree::update (mod.rs:690-701) for distinct leaves as one level-synchronous pass: the resulting tree is
         the one k sequential updates produce, for height device launches instead of k * height."""
+        if self._updates_on_device():
+            self._update_digests(self._check_indexes(indexes), new_leaves)
+            return
         self._apply(*self._updated_nodes(indexes, new_leaves))
 
     def update(self, index: int, new_leaf):
@@ -508,14 +538,12 @@ class MerkleTree:
     def check_update(self, index: int, new_leaf, asserted_new_root) -> bool:
         """mod.rs:706-725: the tree is modified only when the recomputed root equals `asserted_new_root`."""
         assert index < self.leaf_nodes.shape[0], "index out of range"
-        idx, new_hash, changes = self._updated_nodes([index], np.asarray(new_leaf)[None])
-        if not np.array_equal(changes[-1][1][0], np.asarray(asserted_new_root, dtype=np.uint64)):
-            return False
-        self._apply(idx, new_hash, changes)
-        return True
+        return self.check_update_batch([index], np.asarray(new_leaf)[None], asserted_new_root)
 
     def check_update_batch(self, indexes, new_leaves, asserted_new_root) -> bool:
         """check_update for k distinct leaves at once (same acceptance rule, one level-synchronous pass)."""
+        if self._updates_on_device():
+            return self._update_digests(self._check_indexes(indexes), new_leaves, asserted_new_root)
         idx, new_hash, changes = self._updated_nodes(indexes, new_leaves)
         if not np.array_equal(changes[-1][1][0], np.asarray(asserted_new_root, dtype=np.uint64)):
             return False

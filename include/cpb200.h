@@ -76,8 +76,9 @@ typedef struct cpb_multi cpb_multi;         /* a group of GPUs driven by one pro
 
 const char* cpb_last_error(void);
 
-/* ABI revision of this header: bumped when entry points or status codes are added (2 = CPB_INTERNAL_ERROR, cpb_abi_version; 3 = _dev field conversion, host pinning, launch count, multi-GPU build, CPB_NCCL_ERROR, wire formats; 4 = ragged Poseidon batches: CRH, sponge, Merkle build and path verification over inputs of different lengths). */
-#define CPB_ABI_VERSION 4
+/* ABI revision of this header: bumped when entry points or status codes are added (2 = CPB_INTERNAL_ERROR, cpb_abi_version; 3 = _dev field conversion, host pinning, launch count, multi-GPU build, CPB_NCCL_ERROR, wire formats; 4 = ragged Poseidon batches: CRH, sponge, Merkle build and path verification over inputs of different lengths; 5 = Merkle update and
+ * check_update of Poseidon-node trees, in place on device arrays or over host arrays). */
+#define CPB_ABI_VERSION 5
 int cpb_abi_version(void);
 int cpb_version(void);
 /* Number of visible CUDA devices with compute capability 10.x (0 when none / no driver). */
@@ -178,6 +179,39 @@ cpb_status cpb_merkle_poseidon_verify_batch_dev(cpb_poseidon_ctx* leaf_ctx, cpb_
                                                 const uint64_t* leaves, size_t leaf_len, const uint64_t* leaf_sibling_hashes,
                                                 const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes,
                                                 uint8_t* ok, size_t n, void* stream);
+
+/* ---- Merkle tree update (Poseidon inner nodes) ------------------------------------------------------------------ */
+/* k x MerkleTree::update (R/merkle_tree/mod.rs:690-701), or MerkleTree::check_update (:706-725) for all k at once when
+ * asserted_root != NULL, on a tree in the reference's layout: leaf_nodes[n], non_leaf_nodes[n-1] in heap order, updated IN PLACE.
+ * Any tree whose inner hash is poseidon::TwoToOneCRH: field leaves, new_with_leaf_digest / blank trees, and through the digest
+ * form the Pedersen-leaf tree of cpb_merkle_mixed_build (hash the new leaves with cpb_pedersen_crh_x_batch first).
+ * Semantics: the result equals k sequential update(indexes[i], leaf i) calls in input order, so when an index repeats its last
+ * occurrence wins.  With asserted_root the new root is computed first and both arrays are written only when it equals
+ * *asserted_root; otherwise the tree stays bit for bit untouched.  `applied` (nullable) receives 1 when the tree was written
+ * (always, without asserted_root) and 0 otherwise.  asserted_root must not point into the tree.
+ * Rules: n a power of two > 1 (else CPB_NOT_POW2); k >= 2^32 -> CPB_BAD_LENGTH; k == 0 is a no-op returning CPB_OK, `applied` then
+ * says whether the current root equals asserted_root.
+ * The digest forms take new_leaf_digests[k] (leaf digests, e.g. CRH outputs); the leaf forms take new_leaves[k x leaf_len] and hash
+ * all k of them with poseidon::CRH on the same stream first.
+ * _dev forms: every pointer is device memory (`applied` a uint8_t); an index >= n is skipped and nothing outside the caller's arrays
+ * is read or written (indexes are not checked on the host).  No host synchronisation: scratch (about sum over levels l of
+ * min(k, 2^l) elements, at most 2n - 1, plus a few words per index) comes from the stream-ordered pool, and the launches depend on
+ * the tree height only -- one grid per level while a level is wide, one four-warp team launch for the levels above.
+ * Host forms: host arrays, `applied` an int*; an index >= n -> CPB_BAD_PARAMS before any copy.  The tree is not copied: the host
+ * works out which untouched siblings the touched nodes read, uploads those with the indexes and the new leaves, runs the same
+ * device code and copies back only the touched nodes. */
+cpb_status cpb_merkle_poseidon_update_digests_dev(cpb_poseidon_ctx* node_ctx, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes, size_t n,
+                                                  const uint64_t* indexes, const uint64_t* new_leaf_digests, size_t k,
+                                                  const uint64_t* asserted_root, uint8_t* applied, void* stream);
+cpb_status cpb_merkle_poseidon_update_dev(cpb_poseidon_ctx* leaf_ctx, cpb_poseidon_ctx* node_ctx, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes,
+                                          size_t n, const uint64_t* indexes, const uint64_t* new_leaves, size_t leaf_len, size_t k,
+                                          const uint64_t* asserted_root, uint8_t* applied, void* stream);
+cpb_status cpb_merkle_poseidon_update_digests(cpb_poseidon_ctx* node_ctx, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes, size_t n,
+                                              const uint64_t* indexes, const uint64_t* new_leaf_digests, size_t k, const uint64_t* asserted_root,
+                                              int* applied);
+cpb_status cpb_merkle_poseidon_update(cpb_poseidon_ctx* leaf_ctx, cpb_poseidon_ctx* node_ctx, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes,
+                                      size_t n, const uint64_t* indexes, const uint64_t* new_leaves, size_t leaf_len, size_t k,
+                                      const uint64_t* asserted_root, int* applied);
 
 /* ---- Poseidon over inputs of different lengths (ragged batches) --------------------------------------------------- */
 /* The reference's Poseidon input and field leaf are unsized slices (CRHScheme::Input = [F], R/crh/poseidon/mod.rs:19-41;

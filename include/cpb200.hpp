@@ -262,7 +262,37 @@ public:
         return ok;
     }
 
+    // k x MerkleTree::update (mod.rs:690-701) in one call: leaf indexes[i] becomes leaves[i * leaf_len .. (i+1) * leaf_len); a repeated
+    // index takes its last leaf.  Only the touched nodes and the siblings they read cross PCIe.
+    void update_batch(const poseidon::Config& leaf, const poseidon::Config& two_to_one, const std::vector<uint64_t>& indexes,
+                      const std::vector<Fe>& leaves, size_t leaf_len) {
+        update_impl(leaf, two_to_one, indexes, leaves, leaf_len, nullptr);
+    }
+    void update(const poseidon::Config& leaf, const poseidon::Config& two_to_one, size_t index, const std::vector<Fe>& new_leaf) {
+        update_batch(leaf, two_to_one, {(uint64_t)index}, new_leaf, new_leaf.size());
+    }
+    // check_update (mod.rs:706-725) for all k at once: the tree changes only when the new root equals asserted_new_root.
+    bool check_update_batch(const poseidon::Config& leaf, const poseidon::Config& two_to_one, const std::vector<uint64_t>& indexes,
+                            const std::vector<Fe>& leaves, size_t leaf_len, const Fe& asserted_new_root) {
+        return update_impl(leaf, two_to_one, indexes, leaves, leaf_len, &asserted_new_root);
+    }
+    bool check_update(const poseidon::Config& leaf, const poseidon::Config& two_to_one, size_t index, const std::vector<Fe>& new_leaf,
+                      const Fe& asserted_new_root) {
+        return check_update_batch(leaf, two_to_one, {(uint64_t)index}, new_leaf, new_leaf.size(), asserted_new_root);
+    }
+
 private:
+    bool update_impl(const poseidon::Config& leaf, const poseidon::Config& two_to_one, const std::vector<uint64_t>& indexes,
+                     const std::vector<Fe>& leaves, size_t leaf_len, const Fe* asserted) {
+        const size_t k = indexes.size();
+        if (leaves.size() != k * leaf_len) throw Error(CPB_BAD_LENGTH, "one leaf of leaf_len elements per index");
+        int applied = 0;
+        check(cpb_merkle_poseidon_update(leaf.ctx(), two_to_one.ctx(), leaf_nodes.empty() ? nullptr : leaf_nodes[0].data(),
+                                         non_leaf_nodes.empty() ? nullptr : non_leaf_nodes[0].data(), leaf_nodes.size(), indexes.data(),
+                                         leaves.empty() ? nullptr : leaves[0].data(), leaf_len, k, asserted ? asserted->data() : nullptr,
+                                         &applied));
+        return applied != 0;
+    }
     void proofs(const std::vector<size_t>& indexes, std::vector<Fe>& sib, std::vector<Fe>& paths, std::vector<uint64_t>& idx) const {
         const size_t n = indexes.size(), plen = height() - 2;
         sib.resize(n);

@@ -31,6 +31,10 @@ extern "C" {
     fn cpb_poseidon_crh_ragged_batch(ctx: *mut cpb_poseidon_ctx, values: *const u64, offsets: *const u64, out: *mut u64, n: usize) -> c_int;
     fn cpb_merkle_poseidon_build_ragged(leaf: *mut cpb_poseidon_ctx, node: *mut cpb_poseidon_ctx, values: *const u64, offsets: *const u64,
                                         n: usize, leaf_nodes: *mut u64, non_leaf_nodes: *mut u64) -> c_int;
+    // k x MerkleTree::update / check_update on host arrays in place (ABI v5); asserted_root and applied may be null
+    fn cpb_merkle_poseidon_update(leaf: *mut cpb_poseidon_ctx, node: *mut cpb_poseidon_ctx, leaf_nodes: *mut u64, non_leaf_nodes: *mut u64,
+                                  n: usize, indexes: *const u64, new_leaves: *const u64, leaf_len: usize, k: usize,
+                                  asserted_root: *const u64, applied: *mut c_int) -> c_int;
     // page-lock a `Vec<Fr>`'s storage once so the host-pointer calls copy at full PCIe rate (ABI v3)
     fn cpb_host_register(ptr: *mut core::ffi::c_void, bytes: usize) -> c_int;
     fn cpb_host_unregister(ptr: *mut core::ffi::c_void) -> c_int;
@@ -229,6 +233,44 @@ impl<F: GpuField> GpuMerkleTree<F> {
         }
         path.reverse();
         path
+    }
+    /// k x `MerkleTree::update` (R/merkle_tree/mod.rs:690-701) in one call: the touched nodes of every level are hashed on the GPU,
+    /// and only they and the siblings they read cross PCIe.  A repeated index takes its last leaf; new leaves of one length.
+    pub fn update_batch(&mut self, leaf: &GpuPoseidonParams<F>, two_to_one: &GpuPoseidonParams<F>, indexes: &[usize],
+                        new_leaves: &[Vec<F>]) -> Result<(), Error> {
+        self.update_impl(leaf, two_to_one, indexes, new_leaves, None).map(|_| ())
+    }
+    pub fn update(&mut self, leaf: &GpuPoseidonParams<F>, two_to_one: &GpuPoseidonParams<F>, index: usize, new_leaf: &[F]) -> Result<(), Error> {
+        self.update_batch(leaf, two_to_one, &[index], &[new_leaf.to_vec()])
+    }
+    /// `MerkleTree::check_update` (mod.rs:706-725) for all k at once: the tree changes only when the new root equals
+    /// `asserted_new_root`; returns whether it did.
+    pub fn check_update_batch(&mut self, leaf: &GpuPoseidonParams<F>, two_to_one: &GpuPoseidonParams<F>, indexes: &[usize],
+                              new_leaves: &[Vec<F>], asserted_new_root: &F) -> Result<bool, Error> {
+        self.update_impl(leaf, two_to_one, indexes, new_leaves, Some(asserted_new_root))
+    }
+    pub fn check_update(&mut self, leaf: &GpuPoseidonParams<F>, two_to_one: &GpuPoseidonParams<F>, index: usize, new_leaf: &[F],
+                        asserted_new_root: &F) -> Result<bool, Error> {
+        self.check_update_batch(leaf, two_to_one, &[index], &[new_leaf.to_vec()], asserted_new_root)
+    }
+    fn update_impl(&mut self, leaf: &GpuPoseidonParams<F>, two_to_one: &GpuPoseidonParams<F>, indexes: &[usize], new_leaves: &[Vec<F>],
+                   asserted_new_root: Option<&F>) -> Result<bool, Error> {
+        assert_eq!(indexes.len(), new_leaves.len(), "one new leaf per index");
+        let leaf_len = common_len::<_, F>(new_leaves).expect("an update batch takes new leaves of one length");
+        let idx: Vec<u64> = indexes.iter().map(|&i| i as u64).collect();
+        let flat: Vec<u64> = new_leaves.iter().flat_map(|l| flatten(l)).collect();
+        let (mut ln, mut nn) = (flatten(&self.leaf_nodes), flatten(&self.non_leaf_nodes));
+        let root = asserted_new_root.map(|r| r.mont_limbs());
+        let mut applied: c_int = 0;
+        check(unsafe {
+            cpb_merkle_poseidon_update(leaf.ctx.0, two_to_one.ctx.0, ln.as_mut_ptr(), nn.as_mut_ptr(), self.leaf_nodes.len(), idx.as_ptr(),
+                                       flat.as_ptr(), leaf_len, idx.len(), root.as_ref().map_or(core::ptr::null(), |r| r.as_ptr()), &mut applied)
+        })?;
+        if applied != 0 {
+            self.leaf_nodes = unflatten(&ln);
+            self.non_leaf_nodes = unflatten(&nn);
+        }
+        Ok(applied != 0)
     }
 }
 
