@@ -14,9 +14,15 @@ from .crh import poseidon as crh_poseidon
 from .crh import pedersen as crh_pedersen
 from .crh import bowe_hopwood as crh_bowe_hopwood
 from .commitment import pedersen as commitment_pedersen
+from .commitment import blake2s as commitment_blake2s
+from .signature import schnorr as signature_schnorr
+from .signature.schnorr import Schnorr
+from .encryption import elgamal as encryption_elgamal
+from .encryption.elgamal import ElGamal
 from . import curves
 from . import merkle_tree
 
 __all__ = ["Field", "FIELDS", "BLS12_381_FR", "BN254_FR", "JUBJUB_FR", "BLS12_377_FR", "PoseidonConfig", "PoseidonSponge", "absorb_squeeze_batch",
            "absorb_squeeze_ragged",
-           "find_poseidon_ark_and_mds", "get_default_poseidon_parameters", "crh_poseidon", "crh_pedersen", "crh_bowe_hopwood", "commitment_pedersen", "curves", "merkle_tree"]
+           "find_poseidon_ark_and_mds", "get_default_poseidon_parameters", "crh_poseidon", "crh_pedersen", "crh_bowe_hopwood", "commitment_pedersen",
+           "commitment_blake2s", "signature_schnorr", "Schnorr", "encryption_elgamal", "ElGamal", "curves", "merkle_tree"]

@@ -117,6 +117,24 @@ SIGNATURES = {
     "cpb_multi_destroy": (None, [vp]),
     "cpb_multi_uses_nccl": (C.c_int, [vp]),
     "cpb_merkle_poseidon_build_multi": (C.c_int, [vp, C.POINTER(vp), C.POINTER(vp), u64p, C.c_size_t, C.c_size_t, u64p, u64p]),
+    "cpb_te_base_ctx_create": (C.c_int, [C.c_int, u64p, C.c_int, C.POINTER(vp)]),
+    "cpb_te_base_ctx_destroy": (None, [vp]),
+    "cpb_te_base_mul_batch": (C.c_int, [vp, u64p, u64p, C.c_size_t]),
+    "cpb_te_base_mul_batch_dev": (C.c_int, [vp, vp, vp, C.c_size_t, vp]),
+    "cpb_schnorr_sign_batch": (C.c_int, [vp, u8p, u64p, u64p, u8p, u64p, u64p, u8p, C.c_size_t]),
+    "cpb_schnorr_sign_batch_dev": (C.c_int, [vp, u8p, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    "cpb_schnorr_verify_batch": (C.c_int, [vp, u8p, u64p, u8p, u64p, u64p, u8p, C.c_size_t]),
+    "cpb_schnorr_verify_batch_dev": (C.c_int, [vp, u8p, vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    "cpb_schnorr_randomize_public_key_batch": (C.c_int, [vp, u64p, u8p, C.c_size_t, C.c_size_t, u64p, C.c_size_t]),
+    "cpb_schnorr_randomize_public_key_batch_dev": (C.c_int, [vp, vp, vp, C.c_size_t, C.c_size_t, vp, C.c_size_t, vp]),
+    "cpb_schnorr_randomize_signature_batch": (C.c_int, [vp, u64p, u8p, C.c_size_t, C.c_size_t, u64p, C.c_size_t]),
+    "cpb_schnorr_randomize_signature_batch_dev": (C.c_int, [vp, vp, vp, C.c_size_t, C.c_size_t, vp, C.c_size_t, vp]),
+    "cpb_elgamal_encrypt_batch": (C.c_int, [vp, u64p, u64p, u64p, u64p, C.c_size_t]),
+    "cpb_elgamal_encrypt_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    "cpb_elgamal_decrypt_batch": (C.c_int, [vp, u64p, u64p, u64p, C.c_size_t]),
+    "cpb_elgamal_decrypt_batch_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, vp]),
+    "cpb_blake2s_commit_batch": (C.c_int, [C.c_int, u8p, u64p, u8p, u8p, C.c_size_t]),
+    "cpb_blake2s_commit_batch_dev": (C.c_int, [C.c_int, vp, vp, vp, vp, C.c_size_t, vp]),
 }
 
 

@@ -436,6 +436,72 @@ cpb_status cpb_multipath_deserialize(int leaf_kind, int leaf_id, int inner_kind,
                                      uint64_t* suffix_lengths, uint64_t* suffixes, uint64_t* leaf_indexes, size_t cap_paths,
                                      size_t cap_suffix_digests);
 
+/* ---- Schnorr signatures, ElGamal encryption and the Blake2s commitment over Jubjub ------------------------------------ */
+/* signature::schnorr::Schnorr<EdwardsProjective, Blake2s256> (R/signature/schnorr/mod.rs) and encryption::elgamal::ElGamal
+ * (R/encryption/elgamal/mod.rs) for C = ark_ed_on_bls12_381 (Jubjub), the curve of both reference test suites
+ * (R/signature/mod.rs:52-105, R/encryption/elgamal/mod.rs:102-128); commitment::blake2s::Commitment (R/commitment/blake2s/mod.rs).
+ * Layouts: a scalar is an Fr (Jubjub scalar field, CPB_JUBJUB_FR) element as Montgomery limbs, 4 x uint64; a point is affine
+ * x || y, 8 x uint64; a signature is (prover_response s, verifier_challenge e), 8 x uint64; a ciphertext (c1, c2), 16 x uint64.
+ * Messages are ragged bytes: message i = msgs[msg_offsets[i] .. msg_offsets[i+1]), msg_offsets has n + 1 uint64 (the rules of the
+ * ragged Poseidon batches above: host forms reject decreasing offsets with CPB_BAD_LENGTH and copy only msgs[offsets[0] ..
+ * offsets[n]); _dev forms hash a decreasing pair as an empty message).  n >= 2^32 -> CPB_BAD_LENGTH; n == 0 -> CPB_OK, no launch.
+ * PRECONDITIONS.  Public keys, messages and ciphertext points are not checked to be on the curve, and scalars not checked to be
+ * reduced, as for field elements elsewhere.  Secret scalars (sk, nonces, ElGamal randomness) index precomputed tables with
+ * data-dependent addresses: the computation is not constant time (the reference's `mul` is not either).
+ * A _dev call issues several launches on `stream`, takes its scratch from the stream-ordered pool and never synchronises the host. */
+typedef struct cpb_te_base_ctx cpb_te_base_ctx;
+/* Parameters{generator} of both schemes (schnorr/mod.rs:24-29 without the salt, elgamal/mod.rs:14-16), affine (x, y).  Builds the
+ * fixed-base tables of the generator on the device: a Pedersen context (library default chunk width) whose 256 generators are
+ * 2^k G, so s*G is the Pedersen hash of the 32-byte little-endian canonical scalar.  curve_id != CPB_JUBJUB -> CPB_UNSUPPORTED (no
+ * device arithmetic in the scalar field of ed-on-BLS12-377); a generator that is not a reduced point on the curve -> CPB_BAD_PARAMS.
+ * Nothing else is assumed about it: it need not lie in the prime-order subgroup. */
+cpb_status cpb_te_base_ctx_create(int curve_id, const uint64_t* generator_xy, int device, cpb_te_base_ctx** out);
+void cpb_te_base_ctx_destroy(cpb_te_base_ctx* ctx);
+/* keygen of both schemes (schnorr/mod.rs:65-78, elgamal/mod.rs:55-67): out[i] = scalars[i] * G. */
+cpb_status cpb_te_base_mul_batch(cpb_te_base_ctx* ctx, const uint64_t* scalars, uint64_t* out_xy, size_t n);
+cpb_status cpb_te_base_mul_batch_dev(cpb_te_base_ctx* ctx, const uint64_t* scalars, uint64_t* out_xy, size_t n, void* stream);
+/* Schnorr::sign (schnorr/mod.rs:80-115), one loop iteration per item with the given nonce k: R = k*G, e =
+ * Fr::from_random_bytes(Blake2s256(salt || compress(R) || u64_le(len) || msg)), s = k - e*sk.  salt: 32 bytes in HOST memory in both
+ * forms (Parameters.salt), copied into the launch.  signed_out[i] = 0 when the challenge is not a field element (about 9.4 % of
+ * nonces: the digest keeps its low 252 bits and must be below r); the caller draws a new nonce for that item, as the reference's
+ * loop does.  sigs_out[i] is then (0, 0). */
+cpb_status cpb_schnorr_sign_batch(cpb_te_base_ctx* ctx, const uint8_t* salt, const uint64_t* sks, const uint64_t* nonces, const uint8_t* msgs,
+                                  const uint64_t* msg_offsets, uint64_t* sigs_out, uint8_t* signed_out, size_t n);
+cpb_status cpb_schnorr_sign_batch_dev(cpb_te_base_ctx* ctx, const uint8_t* salt, const uint64_t* sks, const uint64_t* nonces, const uint8_t* msgs,
+                                      const uint64_t* msg_offsets, uint64_t* sigs_out, uint8_t* signed_out, size_t n, void* stream);
+/* Schnorr::verify (schnorr/mod.rs:117-148): R' = s*G + e*pk, ok_out[i] = 1 when from_random_bytes(Blake2s256(salt || compress(R') ||
+ * u64_le(len) || msg)) is Some(e') and e' == e. */
+cpb_status cpb_schnorr_verify_batch(cpb_te_base_ctx* ctx, const uint8_t* salt, const uint64_t* pks_xy, const uint8_t* msgs,
+                                    const uint64_t* msg_offsets, const uint64_t* sigs, uint8_t* ok_out, size_t n);
+cpb_status cpb_schnorr_verify_batch_dev(cpb_te_base_ctx* ctx, const uint8_t* salt, const uint64_t* pks_xy, const uint8_t* msgs,
+                                        const uint64_t* msg_offsets, const uint64_t* sigs, uint8_t* ok_out, size_t n, void* stream);
+/* Schnorr::randomize_public_key (schnorr/mod.rs:150-174): out[i] = pk[i] + m*G with m = sum_b bitrev8(byte_b) 2^(8b) over the `len`
+ * bytes at randomness + i*stride (bytes_to_bits, :185-194, read as little-endian bits), the exact integer of any length, not reduced
+ * mod r.  len >= 2^24 -> CPB_BAD_LENGTH; host forms: len > stride (n > 1) -> CPB_BAD_LENGTH. */
+cpb_status cpb_schnorr_randomize_public_key_batch(cpb_te_base_ctx* ctx, const uint64_t* pks_xy, const uint8_t* randomness, size_t len,
+                                                  size_t stride, uint64_t* out_xy, size_t n);
+cpb_status cpb_schnorr_randomize_public_key_batch_dev(cpb_te_base_ctx* ctx, const uint64_t* pks_xy, const uint8_t* randomness, size_t len,
+                                                      size_t stride, uint64_t* out_xy, size_t n, void* stream);
+/* Schnorr::randomize_signature (schnorr/mod.rs:176-198): (s - e*m, e) in Fr, m as above reduced mod r. */
+cpb_status cpb_schnorr_randomize_signature_batch(cpb_te_base_ctx* ctx, const uint64_t* sigs, const uint8_t* randomness, size_t len,
+                                                 size_t stride, uint64_t* sigs_out, size_t n);
+cpb_status cpb_schnorr_randomize_signature_batch_dev(cpb_te_base_ctx* ctx, const uint64_t* sigs, const uint8_t* randomness, size_t len,
+                                                     size_t stride, uint64_t* sigs_out, size_t n, void* stream);
+/* ElGamal::encrypt (elgamal/mod.rs:69-84): (r*G, m + r*pk); ElGamal::decrypt (:86-101): c2 - sk*c1. */
+cpb_status cpb_elgamal_encrypt_batch(cpb_te_base_ctx* ctx, const uint64_t* pks_xy, const uint64_t* msgs_xy, const uint64_t* rands,
+                                     uint64_t* ciphertexts_out, size_t n);
+cpb_status cpb_elgamal_encrypt_batch_dev(cpb_te_base_ctx* ctx, const uint64_t* pks_xy, const uint64_t* msgs_xy, const uint64_t* rands,
+                                         uint64_t* ciphertexts_out, size_t n, void* stream);
+cpb_status cpb_elgamal_decrypt_batch(cpb_te_base_ctx* ctx, const uint64_t* sks, const uint64_t* ciphertexts, uint64_t* msgs_out, size_t n);
+cpb_status cpb_elgamal_decrypt_batch_dev(cpb_te_base_ctx* ctx, const uint64_t* sks, const uint64_t* ciphertexts, uint64_t* msgs_out, size_t n,
+                                         void* stream);
+/* commitment::blake2s::Commitment::commit (R/commitment/blake2s/mod.rs:21-32): out32[i] = Blake2s256(input_i || randomness32[i]);
+ * inputs are ragged bytes under the message rules above. */
+cpb_status cpb_blake2s_commit_batch(int device, const uint8_t* in, const uint64_t* offsets, const uint8_t* randomness32, uint8_t* out32,
+                                    size_t n);
+cpb_status cpb_blake2s_commit_batch_dev(int device, const uint8_t* in, const uint64_t* offsets, const uint8_t* randomness32, uint8_t* out32,
+                                        size_t n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

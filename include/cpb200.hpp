@@ -185,6 +185,146 @@ struct Commitment {   // R/commitment/pedersen/mod.rs:38-106; randomness = 32-by
 
 }  // namespace pedersen
 
+// Byte strings of different lengths as the C-ABI's ragged batch: the bytes back to back plus n + 1 offsets.
+inline void ragged_pack(const std::vector<std::vector<uint8_t>>& inputs, std::vector<uint8_t>& values, std::vector<uint64_t>& offsets) {
+    offsets.assign(1, 0);
+    values.clear();
+    for (const auto& x : inputs) {
+        values.insert(values.end(), x.begin(), x.end());
+        offsets.push_back(values.size());
+    }
+    values.push_back(0);                                  // never empty, so data() is a valid pointer
+}
+
+// Parameters{generator} shared by Schnorr and ElGamal over Jubjub, with the generator's fixed-base tables on the device.
+class TeBase {
+public:
+    Affine generator;
+    explicit TeBase(const Affine& g, int curve = CPB_JUBJUB, int device = 0) : generator(g) {
+        cpb_te_base_ctx* c = nullptr;
+        check(cpb_te_base_ctx_create(curve, g.x.data(), device, &c));
+        ctx_.reset(c, cpb_te_base_ctx_destroy);
+    }
+    cpb_te_base_ctx* ctx() const { return ctx_.get(); }
+    // keygen of both schemes: scalars[i] * generator (Fr Montgomery limbs)
+    std::vector<Affine> mul_batch(const std::vector<Fe>& scalars) const {
+        std::vector<Affine> out(scalars.size());
+        if (!scalars.empty()) check(cpb_te_base_mul_batch(ctx(), scalars[0].data(), out[0].x.data(), scalars.size()));
+        return out;
+    }
+
+private:
+    std::shared_ptr<cpb_te_base_ctx> ctx_;
+};
+
+namespace schnorr {   // Schnorr<Jubjub, Blake2s256>, R/signature/schnorr/mod.rs; SignatureScheme, R/signature/mod.rs:14-50
+
+struct Signature { Fe prover_response, verifier_challenge; };
+
+// schnorr::Parameters{generator, salt} (mod.rs:24-29)
+struct Parameters {
+    TeBase base;
+    std::array<uint8_t, 32> salt;
+    Parameters(const Affine& generator, const std::array<uint8_t, 32>& salt_, int device = 0) : base(generator, CPB_JUBJUB, device), salt(salt_) {}
+};
+
+struct Schnorr {
+    static std::vector<Affine> keygen_batch(const Parameters& p, const std::vector<Fe>& secret_keys) { return p.base.mul_batch(secret_keys); }
+    // One iteration of the signing loop (mod.rs:87-104) per item with the given nonce; signed[i] = 0 when the challenge is not
+    // a field element -- draw a new nonce for that item.
+    static std::vector<Signature> sign_with_nonces_batch(const Parameters& p, const std::vector<Fe>& sks, const std::vector<Fe>& nonces,
+                                                         const std::vector<std::vector<uint8_t>>& messages, std::vector<uint8_t>& signed_out) {
+        const size_t n = sks.size();
+        if (nonces.size() != n || messages.size() != n) throw Error(CPB_BAD_LENGTH, "sign: one nonce and one message per key");
+        std::vector<uint8_t> values;
+        std::vector<uint64_t> offsets;
+        ragged_pack(messages, values, offsets);
+        std::vector<Signature> out(n);
+        signed_out.assign(n, 0);
+        if (n) check(cpb_schnorr_sign_batch(p.base.ctx(), p.salt.data(), sks[0].data(), nonces[0].data(), values.data(), offsets.data(),
+                                            out[0].prover_response.data(), signed_out.data(), n));
+        return out;
+    }
+    // mod.rs:117-148
+    static std::vector<uint8_t> verify_batch(const Parameters& p, const std::vector<Affine>& pks, const std::vector<std::vector<uint8_t>>& messages,
+                                             const std::vector<Signature>& sigs) {
+        const size_t n = pks.size();
+        if (messages.size() != n || sigs.size() != n) throw Error(CPB_BAD_LENGTH, "verify: one message and one signature per key");
+        std::vector<uint8_t> values, ok(n);
+        std::vector<uint64_t> offsets;
+        ragged_pack(messages, values, offsets);
+        if (n) check(cpb_schnorr_verify_batch(p.base.ctx(), p.salt.data(), pks[0].x.data(), values.data(), offsets.data(),
+                                              sigs[0].prover_response.data(), ok.data(), n));
+        return ok;
+    }
+    static bool verify(const Parameters& p, const Affine& pk, const std::vector<uint8_t>& message, const Signature& sig) {
+        return verify_batch(p, {pk}, {message}, {sig})[0] != 0;
+    }
+    // mod.rs:150-174; randomness: n x len bytes
+    static std::vector<Affine> randomize_public_key_batch(const Parameters& p, const std::vector<Affine>& pks, const uint8_t* randomness, size_t len) {
+        std::vector<Affine> out(pks.size());
+        if (!pks.empty())
+            check(cpb_schnorr_randomize_public_key_batch(p.base.ctx(), pks[0].x.data(), randomness, len, len, out[0].x.data(), pks.size()));
+        return out;
+    }
+    // mod.rs:176-198
+    static std::vector<Signature> randomize_signature_batch(const Parameters& p, const std::vector<Signature>& sigs, const uint8_t* randomness,
+                                                            size_t len) {
+        std::vector<Signature> out(sigs.size());
+        if (!sigs.empty())
+            check(cpb_schnorr_randomize_signature_batch(p.base.ctx(), sigs[0].prover_response.data(), randomness, len, len,
+                                                        out[0].prover_response.data(), sigs.size()));
+        return out;
+    }
+};
+
+}  // namespace schnorr
+
+namespace elgamal {   // ElGamal<Jubjub>, R/encryption/elgamal/mod.rs; AsymmetricEncryptionScheme
+
+struct Ciphertext { Affine c1, c2; };
+using Parameters = TeBase;   // elgamal::Parameters{generator} (mod.rs:14-16)
+
+struct ElGamal {
+    // mod.rs:69-84
+    static std::vector<Ciphertext> encrypt_batch(const Parameters& p, const std::vector<Affine>& pks, const std::vector<Affine>& msgs,
+                                                 const std::vector<Fe>& rands) {
+        const size_t n = pks.size();
+        if (msgs.size() != n || rands.size() != n) throw Error(CPB_BAD_LENGTH, "encrypt: one message and one randomness per key");
+        std::vector<Ciphertext> out(n);
+        if (n) check(cpb_elgamal_encrypt_batch(p.ctx(), pks[0].x.data(), msgs[0].x.data(), rands[0].data(), out[0].c1.x.data(), n));
+        return out;
+    }
+    // mod.rs:86-101
+    static std::vector<Affine> decrypt_batch(const Parameters& p, const std::vector<Fe>& sks, const std::vector<Ciphertext>& cts) {
+        const size_t n = sks.size();
+        if (cts.size() != n) throw Error(CPB_BAD_LENGTH, "decrypt: one ciphertext per key");
+        std::vector<Affine> out(n);
+        if (n) check(cpb_elgamal_decrypt_batch(p.ctx(), sks[0].data(), cts[0].c1.x.data(), out[0].x.data(), n));
+        return out;
+    }
+};
+
+}  // namespace elgamal
+
+namespace blake2s {   // commitment::blake2s::Commitment, R/commitment/blake2s/mod.rs:11-33
+
+struct Commitment {
+    static std::vector<std::array<uint8_t, 32>> commit_batch(const std::vector<std::vector<uint8_t>>& inputs,
+                                                             const std::vector<std::array<uint8_t, 32>>& randomness, int device = 0) {
+        const size_t n = inputs.size();
+        if (randomness.size() != n) throw Error(CPB_BAD_LENGTH, "commit: one randomness per input");
+        std::vector<uint8_t> values;
+        std::vector<uint64_t> offsets;
+        ragged_pack(inputs, values, offsets);
+        std::vector<std::array<uint8_t, 32>> out(n);
+        if (n) check(cpb_blake2s_commit_batch(device, values.data(), offsets.data(), randomness[0].data(), out[0].data(), n));
+        return out;
+    }
+};
+
+}  // namespace blake2s
+
 // MerkleTree<FieldMTConfig> (R/merkle_tree/mod.rs:381-533; Config of R/merkle_tree/tests/mod.rs:198-206)
 class PoseidonMerkleTree {
 public:

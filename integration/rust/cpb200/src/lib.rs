@@ -428,3 +428,209 @@ pub mod pedersen {
         }
     }
 }
+
+/// `signature::schnorr::Schnorr<EdwardsProjective, Blake2s256>` and `encryption::elgamal::ElGamal<EdwardsProjective>` over Jubjub
+/// (R/signature/schnorr/mod.rs, R/encryption/elgamal/mod.rs) on `cpb_te_base_ctx`.  SOURCE ONLY, like the rest of this crate.
+/// Keys and signatures are the reference's own types, so a key pair or signature made here verifies with the reference and
+/// the other way round.  Signing is not constant time (secret scalars select table entries by value), as the reference's.
+pub mod signature {
+    use super::{check, GpuField};
+    use ark_crypto_primitives::encryption::{elgamal as ref_eg, AsymmetricEncryptionScheme};
+    use ark_crypto_primitives::signature::{schnorr as ref_sig, SignatureScheme};
+    use ark_crypto_primitives::Error;
+    use ark_ec::AffineRepr;
+    use ark_ed_on_bls12_381::{EdwardsAffine, EdwardsProjective, Fq, Fr};
+    use ark_std::{rand::Rng, sync::Arc, UniformRand};
+    use blake2::Blake2s256;
+    use std::os::raw::c_int;
+
+    #[allow(non_camel_case_types)]
+    #[repr(C)]
+    pub struct cpb_te_base_ctx {
+        _private: [u8; 0],
+    }
+    extern "C" {
+        fn cpb_te_base_ctx_create(curve_id: c_int, generator_xy: *const u64, device: c_int, out: *mut *mut cpb_te_base_ctx) -> c_int;
+        fn cpb_te_base_ctx_destroy(ctx: *mut cpb_te_base_ctx);
+        fn cpb_te_base_mul_batch(ctx: *mut cpb_te_base_ctx, scalars: *const u64, out_xy: *mut u64, n: usize) -> c_int;
+        fn cpb_schnorr_sign_batch(ctx: *mut cpb_te_base_ctx, salt: *const u8, sks: *const u64, nonces: *const u64, msgs: *const u8,
+                                  msg_offsets: *const u64, sigs_out: *mut u64, signed_out: *mut u8, n: usize) -> c_int;
+        fn cpb_schnorr_verify_batch(ctx: *mut cpb_te_base_ctx, salt: *const u8, pks_xy: *const u64, msgs: *const u8, msg_offsets: *const u64,
+                                    sigs: *const u64, ok_out: *mut u8, n: usize) -> c_int;
+        fn cpb_schnorr_randomize_public_key_batch(ctx: *mut cpb_te_base_ctx, pks_xy: *const u64, randomness: *const u8, len: usize,
+                                                  stride: usize, out_xy: *mut u64, n: usize) -> c_int;
+        fn cpb_schnorr_randomize_signature_batch(ctx: *mut cpb_te_base_ctx, sigs: *const u64, randomness: *const u8, len: usize,
+                                                 stride: usize, sigs_out: *mut u64, n: usize) -> c_int;
+        fn cpb_elgamal_encrypt_batch(ctx: *mut cpb_te_base_ctx, pks_xy: *const u64, msgs_xy: *const u64, rands: *const u64,
+                                     ciphertexts_out: *mut u64, n: usize) -> c_int;
+        fn cpb_elgamal_decrypt_batch(ctx: *mut cpb_te_base_ctx, sks: *const u64, ciphertexts: *const u64, msgs_out: *mut u64, n: usize) -> c_int;
+    }
+
+    struct Ctx(*mut cpb_te_base_ctx);
+    unsafe impl Send for Ctx {}
+    unsafe impl Sync for Ctx {}
+    impl Drop for Ctx {
+        fn drop(&mut self) { unsafe { cpb_te_base_ctx_destroy(self.0) } }
+    }
+
+    fn xy(p: &EdwardsAffine) -> [u64; 8] {
+        let (x, y) = p.xy().unwrap_or((Fq::from(0u64), Fq::from(1u64)));     // the identity is (0, 1)
+        let mut out = [0u64; 8];
+        out[..4].copy_from_slice(&x.mont_limbs());
+        out[4..].copy_from_slice(&y.mont_limbs());
+        out
+    }
+    fn point(l: &[u64]) -> EdwardsAffine {
+        EdwardsAffine::new_unchecked(Fq::from_mont_limbs([l[0], l[1], l[2], l[3]]), Fq::from_mont_limbs([l[4], l[5], l[6], l[7]]))
+    }
+
+    /// A generator and its device tables (`cpb_te_base_ctx`).
+    #[derive(Clone)]
+    pub struct GpuBase {
+        pub generator: EdwardsAffine,
+        ctx: Arc<Ctx>,
+    }
+    impl GpuBase {
+        pub fn new(generator: EdwardsAffine, device: i32) -> Result<Self, Error> {
+            let g = xy(&generator);
+            let mut raw = core::ptr::null_mut();
+            check(unsafe { cpb_te_base_ctx_create(0, g.as_ptr(), device, &mut raw) })?;
+            Ok(Self { generator, ctx: Arc::new(Ctx(raw)) })
+        }
+        fn mul(&self, s: &Fr) -> Result<EdwardsAffine, Error> {
+            let mut out = [0u64; 8];
+            check(unsafe { cpb_te_base_mul_batch(self.ctx.0, s.mont_limbs().as_ptr(), out.as_mut_ptr(), 1) })?;
+            Ok(point(&out))
+        }
+    }
+
+    /// `schnorr::Parameters` + device tables.
+    #[derive(Clone)]
+    pub struct GpuSchnorrParams {
+        pub base: GpuBase,
+        pub salt: [u8; 32],
+    }
+    impl GpuSchnorrParams {
+        pub fn from_reference(p: &ref_sig::Parameters<EdwardsProjective, Blake2s256>, device: i32) -> Result<Self, Error> {
+            Ok(Self { base: GpuBase::new(p.generator, device)?, salt: p.salt })
+        }
+    }
+
+    fn sig_limbs(s: &ref_sig::Signature<EdwardsProjective>) -> [u64; 8] {
+        let mut out = [0u64; 8];
+        out[..4].copy_from_slice(&s.prover_response.mont_limbs());
+        out[4..].copy_from_slice(&s.verifier_challenge.mont_limbs());
+        out
+    }
+    fn sig_from(l: &[u64]) -> ref_sig::Signature<EdwardsProjective> {
+        ref_sig::Signature {
+            prover_response: Fr::from_mont_limbs([l[0], l[1], l[2], l[3]]),
+            verifier_challenge: Fr::from_mont_limbs([l[4], l[5], l[6], l[7]]),
+        }
+    }
+
+    pub struct GpuSchnorr;
+    impl GpuSchnorr {
+        /// Many messages at once: one verification per (pk, message, signature), one device call.
+        pub fn verify_batch(pp: &GpuSchnorrParams, pks: &[EdwardsAffine], messages: &[&[u8]], sigs: &[ref_sig::Signature<EdwardsProjective>])
+                            -> Result<Vec<bool>, Error> {
+            let n = pks.len();
+            assert!(messages.len() == n && sigs.len() == n);
+            let pk: Vec<u64> = pks.iter().flat_map(xy).collect();
+            let sg: Vec<u64> = sigs.iter().flat_map(sig_limbs).collect();
+            let mut values: Vec<u8> = messages.concat();
+            values.push(0);
+            let mut off = vec![0u64];
+            for m in messages {
+                off.push(off[off.len() - 1] + m.len() as u64);
+            }
+            let mut ok = vec![0u8; n];
+            check(unsafe {
+                cpb_schnorr_verify_batch(pp.base.ctx.0, pp.salt.as_ptr(), pk.as_ptr(), values.as_ptr(), off.as_ptr(), sg.as_ptr(), ok.as_mut_ptr(), n)
+            })?;
+            Ok(ok.into_iter().map(|b| b != 0).collect())
+        }
+    }
+    impl SignatureScheme for GpuSchnorr {
+        type Parameters = GpuSchnorrParams;
+        type PublicKey = EdwardsAffine;
+        type SecretKey = ref_sig::SecretKey<EdwardsProjective>;
+        type Signature = ref_sig::Signature<EdwardsProjective>;
+
+        fn setup<R: Rng>(rng: &mut R) -> Result<Self::Parameters, Error> {
+            GpuSchnorrParams::from_reference(&ref_sig::Schnorr::<EdwardsProjective, Blake2s256>::setup(rng)?, 0)
+        }
+        fn keygen<R: Rng>(pp: &Self::Parameters, rng: &mut R) -> Result<(Self::PublicKey, Self::SecretKey), Error> {
+            let sk = Fr::rand(rng);
+            Ok((pp.base.mul(&sk)?, ref_sig::SecretKey(sk)))
+        }
+        /// mod.rs:80-115: draw a nonce, one device call, redraw while the challenge is not a field element.
+        fn sign<R: Rng>(pp: &Self::Parameters, sk: &Self::SecretKey, message: &[u8], rng: &mut R) -> Result<Self::Signature, Error> {
+            let off = [0u64, message.len() as u64];
+            let mut values = message.to_vec();
+            values.push(0);
+            loop {
+                let k = Fr::rand(rng);
+                let (mut sig, mut signed) = ([0u64; 8], 0u8);
+                check(unsafe {
+                    cpb_schnorr_sign_batch(pp.base.ctx.0, pp.salt.as_ptr(), sk.0.mont_limbs().as_ptr(), k.mont_limbs().as_ptr(), values.as_ptr(),
+                                           off.as_ptr(), sig.as_mut_ptr(), &mut signed, 1)
+                })?;
+                if signed != 0 {
+                    return Ok(sig_from(&sig));
+                }
+            }
+        }
+        fn verify(pp: &Self::Parameters, pk: &Self::PublicKey, message: &[u8], signature: &Self::Signature) -> Result<bool, Error> {
+            Ok(GpuSchnorr::verify_batch(pp, &[*pk], &[message], core::slice::from_ref(signature))?[0])
+        }
+        fn randomize_public_key(pp: &Self::Parameters, public_key: &Self::PublicKey, randomness: &[u8]) -> Result<Self::PublicKey, Error> {
+            let (pk, mut out) = (xy(public_key), [0u64; 8]);
+            check(unsafe {
+                cpb_schnorr_randomize_public_key_batch(pp.base.ctx.0, pk.as_ptr(), randomness.as_ptr(), randomness.len(), randomness.len(),
+                                                       out.as_mut_ptr(), 1)
+            })?;
+            Ok(point(&out))
+        }
+        fn randomize_signature(pp: &Self::Parameters, signature: &Self::Signature, randomness: &[u8]) -> Result<Self::Signature, Error> {
+            let (sg, mut out) = (sig_limbs(signature), [0u64; 8]);
+            check(unsafe {
+                cpb_schnorr_randomize_signature_batch(pp.base.ctx.0, sg.as_ptr(), randomness.as_ptr(), randomness.len(), randomness.len(),
+                                                      out.as_mut_ptr(), 1)
+            })?;
+            Ok(sig_from(&out))
+        }
+    }
+
+    /// `encryption::elgamal::ElGamal<EdwardsProjective>` (R/encryption/elgamal/mod.rs:34-101).
+    pub struct GpuElGamal;
+    impl AsymmetricEncryptionScheme for GpuElGamal {
+        type Parameters = GpuBase;
+        type PublicKey = EdwardsAffine;
+        type SecretKey = ref_eg::SecretKey<EdwardsProjective>;
+        type Randomness = ref_eg::Randomness<EdwardsProjective>;
+        type Plaintext = EdwardsAffine;
+        type Ciphertext = (EdwardsAffine, EdwardsAffine);
+
+        fn setup<R: Rng>(rng: &mut R) -> Result<Self::Parameters, Error> {
+            GpuBase::new(ref_eg::ElGamal::<EdwardsProjective>::setup(rng)?.generator, 0)
+        }
+        fn keygen<R: Rng>(pp: &Self::Parameters, rng: &mut R) -> Result<(Self::PublicKey, Self::SecretKey), Error> {
+            let sk = Fr::rand(rng);
+            Ok((pp.mul(&sk)?, ref_eg::SecretKey(sk)))
+        }
+        fn encrypt(pp: &Self::Parameters, pk: &Self::PublicKey, message: &Self::Plaintext, r: &Self::Randomness) -> Result<Self::Ciphertext, Error> {
+            let (p, m, mut out) = (xy(pk), xy(message), [0u64; 16]);
+            check(unsafe { cpb_elgamal_encrypt_batch(pp.ctx.0, p.as_ptr(), m.as_ptr(), r.0.mont_limbs().as_ptr(), out.as_mut_ptr(), 1) })?;
+            Ok((point(&out[..8]), point(&out[8..])))
+        }
+        fn decrypt(pp: &Self::Parameters, sk: &Self::SecretKey, ciphertext: &Self::Ciphertext) -> Result<Self::Plaintext, Error> {
+            let mut ct = [0u64; 16];
+            ct[..8].copy_from_slice(&xy(&ciphertext.0));
+            ct[8..].copy_from_slice(&xy(&ciphertext.1));
+            let mut out = [0u64; 8];
+            check(unsafe { cpb_elgamal_decrypt_batch(pp.ctx.0, sk.0.mont_limbs().as_ptr(), ct.as_ptr(), out.as_mut_ptr(), 1) })?;
+            Ok(point(&out))
+        }
+    }
+}
