@@ -84,6 +84,10 @@ SIGNATURES = {
     "cpb_bowe_hopwood_two_to_one_scratch_bytes": (C.c_size_t, [vp, C.c_size_t]),
     "cpb_merkle_pedersen_build": (C.c_int, [vp, vp, u8p, C.c_size_t, C.c_size_t, u64p, u64p]),
     "cpb_merkle_pedersen_build_dev": (C.c_int, [vp, vp, vp, C.c_size_t, C.c_size_t, C.c_size_t, vp, vp, vp, vp]),
+    "cpb_merkle_pedersen_update_digests_dev": (C.c_int, [vp, vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp, vp, vp]),
+    "cpb_merkle_pedersen_update_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, vp, vp, C.c_size_t, C.c_size_t, C.c_size_t, vp, vp, vp]),
+    "cpb_merkle_pedersen_update_digests": (C.c_int, [vp, u64p, u64p, C.c_size_t, u64p, u64p, C.c_size_t, u64p, C.POINTER(C.c_int)]),
+    "cpb_merkle_pedersen_update": (C.c_int, [vp, vp, u64p, u64p, C.c_size_t, u64p, u8p, C.c_size_t, C.c_size_t, u64p, C.POINTER(C.c_int)]),
     "cpb_merkle_mixed_build": (C.c_int, [vp, vp, u8p, C.c_size_t, C.c_size_t, u64p, u64p]),
     "cpb_merkle_mixed_build_dev": (C.c_int, [vp, vp, vp, C.c_size_t, C.c_size_t, C.c_size_t, vp, vp, vp]),
     "cpb_exchange_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),

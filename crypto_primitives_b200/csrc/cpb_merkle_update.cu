@@ -11,59 +11,17 @@
 //             so no CTA ever waits for another
 //   commit    one grid scatters the scratch into the tree, predicated on the device-side comparison with asserted_root
 // The launch count depends on the tree height only.  Scratch comes from the stream-ordered pool; nothing synchronises the host.
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
-
-#include <cstring>
-#include <vector>
-
 #include "merkle_update.cuh"
+#include "merkle_update_kernels.cuh"
 #include "poseidon_kernels.cuh"
 
 namespace cpb {
 namespace {
 
-constexpr int kUpdBlock = 256;
-
-unsigned upd_grid(u64 items, int block) { return (unsigned)((items + block - 1) / block); }
-
-__global__ void k_upd_keys(const u64* __restrict__ idx, u64 k, u64 n, u64* __restrict__ keys, unsigned* __restrict__ pos) {
-    const u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= k) return;
-    const u64 v = idx[j];
-    keys[j] = v < n ? v : n;                                   // out of range: sorts last, dropped by k_upd_flags
-    pos[j] = (unsigned)j;
-}
-
-// Keep the last occurrence of every in-range index.
-__global__ void k_upd_flags(const u64* __restrict__ K, u64 k, u64 n, unsigned* __restrict__ flag) {
-    const u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= k) return;
-    flag[j] = K[j] < n && (j + 1 == k || K[j + 1] != K[j]) ? 1u : 0u;
-}
-
-// U[scan[j]] = K[j] for the kept j, the digest of input pos[j] into the leaf level of the scratch, m = the number kept.
-__global__ void k_upd_compact(const u64* __restrict__ K, const unsigned* __restrict__ pos, const unsigned* __restrict__ flag,
-                              const unsigned* __restrict__ scan, u64 k, int h, const u32* __restrict__ digests, u64* __restrict__ U,
-                              u64* __restrict__ m, u32* __restrict__ leaf_scratch) {
-    const u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= k) return;
-    if (j + 1 == k) *m = (u64)scan[j] + flag[j];
-    if (!flag[j]) return;
-    const u64 i = scan[j];
-    U[i] = K[j];
-    u32 e[8];
-    ld_elem(e, digests + 8 * (u64)pos[j]);
-    st_elem(leaf_scratch + 8 * (upd_dense(h, k) ? K[j] : i), e);
-}
-
-// Where the current value of child `node` (level l + 1) of a touched node of level l is: the scratch when the child is touched
-// too, the caller's tree otherwise.
+// Where the current value of child `node` (level l + 1) of a touched node of level l is (merkle_update.cuh, upd_child_at).
 __device__ __forceinline__ const u32* upd_child(const UpdPlan& X, int l, bool touched, u64 slot, u64 node, const u32* scratch,
                                                 const u32* leaf_nodes, const u32* nodes) {
-    if (touched) return scratch + 8 * (X.off[l + 1] + slot);
-    if (l + 1 == X.h) return leaf_nodes + 8 * node;
-    return nodes + 8 * (((1ull << (l + 1)) - 1) + node);
+    return upd_child_at<8>(X, l, touched, slot, node, scratch, leaf_nodes, nodes);
 }
 
 // One level, one candidate per thread; only touched candidates hash.
@@ -151,38 +109,6 @@ k_merkle_update_top(PoseidonDev P, const u32* __restrict__ consts, UpdPlan X, in
     }
 }
 
-// applied = (asserted == NULL or new root == asserted); when applied, every touched node's new value goes into the tree.
-// X.m == NULL: nothing is touched (k == 0), the new root is the current one.
-__global__ void k_upd_commit(UpdPlan X, const u32* __restrict__ scratch, u32* leaf_nodes, u32* nodes, const u32* __restrict__ asserted,
-                             unsigned char* __restrict__ applied) {
-    const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    const u64 m = X.m ? *X.m : 0;
-    bool ok = true;
-    if (asserted) {
-        u32 r[8], a[8];
-        ld_elem(r, m ? scratch + 8 * X.off[0] : nodes);
-        ld_elem(a, asserted);
-        ok = fp_eq(r, a);
-    }
-    if (t == 0 && applied) *applied = ok ? 1 : 0;
-    if (!ok || m == 0 || t >= X.off[X.h + 1]) return;
-    const int l = upd_level_of(X.off, X.h, t);
-    const UpdSite S = upd_site(X.U, m, X.h, l, X.k, t - X.off[l]);
-    if (!S.touched) return;
-    u32 e[8];
-    ld_elem(e, scratch + 8 * t);                               // slot t - off[l] of level l
-    st_elem(l == X.h ? leaf_nodes + 8 * S.node : nodes + 8 * (((1ull << l) - 1) + S.node), e);
-}
-
-// dst[pos[i]] = src[i] (scatter) or dst[i] = src[pos[i]] (gather), elements.
-__global__ void k_upd_move(const u32* __restrict__ src, u32* __restrict__ dst, const u64* __restrict__ pos, u64 cnt, int gather) {
-    const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= cnt) return;
-    u32 e[8];
-    ld_elem(e, src + 8 * (gather ? pos[i] : i));
-    st_elem(dst + 8 * (gather ? i : pos[i]), e);
-}
-
 template <class F, int T>
 cpb_status launch_level_ft(cpb_poseidon_ctx* c, const UpdPlan& X, int l, u32* scratch, const u32* leaf_nodes, const u32* nodes,
                            cudaStream_t st) {
@@ -254,12 +180,6 @@ cpb_status launch_top(cpb_poseidon_ctx* c, const UpdPlan& X, int l, u32* scratch
     return fail(CPB_BAD_PARAMS, "unknown field id %d", c->field_id);
 }
 
-int log2_exact(size_t n) {
-    int h = 0;
-    while (((size_t)1 << h) < n) h++;
-    return h;
-}
-
 // Highest level the team launch starts at (-1: every level gets a grid of its own).  Level widths shrink towards the root, so
 // every level above it fits too.
 int team_start_level(const cpb_poseidon_ctx* node, int h, u64 k) {
@@ -278,78 +198,35 @@ cpb_status update_digests_dev(cpb_poseidon_ctx* node, u32* leaf_nodes, u32* node
     upd_offsets(X.h, k, X.off);
     if (k == 0) {
         if (applied) {
-            k_upd_commit<<<1, 32, 0, st>>>(X, nullptr, leaf_nodes, nodes, asserted, applied);
+            k_upd_commit<8><<<1, 32, 0, st>>>(X, nullptr, leaf_nodes, nodes, asserted, applied);
             CPB_CUDA(cudaGetLastError());
         }
         return CPB_OK;
     }
     const int lt = team_start_level(node, X.h, k);
-    const unsigned uk = (unsigned)k;
-    size_t sort_b = 0, scan_b = 0;
-    CPB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const u64*)nullptr, (u64*)nullptr, (const unsigned*)nullptr, (unsigned*)nullptr,
-                                             uk, 0, X.h + 1, st));
-    CPB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const unsigned*)nullptr, (unsigned*)nullptr, uk, st));
-    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t tmp_b = sort_b > scan_b ? sort_b : scan_b;
     const size_t n_arr = lt >= 0 ? (size_t)X.off[lt] : 0;      // arrival counters of the levels above the team start
-    size_t o = 0;
-    const size_t o_kin = o; o += up(8 * k);
-    const size_t o_kout = o; o += up(8 * k);
-    const size_t o_pin = o; o += up(4 * k);
-    const size_t o_pout = o; o += up(4 * k);
-    const size_t o_flag = o; o += up(4 * k);
-    const size_t o_scan = o; o += up(4 * k);
-    const size_t o_U = o; o += up(8 * k);
-    const size_t o_m = o; o += 256;
-    const size_t o_tmp = o; o += up(tmp_b);
-    const size_t o_arr = o; o += up(4 * n_arr + 4);
-    const size_t o_scr = o; o += 32 * (size_t)X.off[X.h + 1];
-    char* b = nullptr;
-    CPB_CUDA(cudaMallocAsync((void**)&b, o, st));
+    UpdBuffers B;
+    CPB_TRY(upd_layout(X, n, k, 4 * n_arr + 4, 8, st, B));
+    CPB_CUDA(cudaMallocAsync((void**)&B.b, B.total, st));
     auto run = [&]() -> cpb_status {
-        u64* kin = (u64*)(b + o_kin);
-        u64* kout = (u64*)(b + o_kout);
-        unsigned* pin = (unsigned*)(b + o_pin);
-        unsigned* pout = (unsigned*)(b + o_pout);
-        unsigned* flag = (unsigned*)(b + o_flag);
-        unsigned* scan = (unsigned*)(b + o_scan);
-        u32* scratch = (u32*)(b + o_scr);
-        X.U = (const u64*)(b + o_U);
-        X.m = (const u64*)(b + o_m);
-        const unsigned g = upd_grid(k, kUpdBlock);
-        k_upd_keys<<<g, kUpdBlock, 0, st>>>(idx, k, n, kin, pin);
-        CPB_CUDA(cudaGetLastError());
-        size_t tb = tmp_b;
-        CPB_CUDA(cub::DeviceRadixSort::SortPairs(b + o_tmp, tb, (const u64*)kin, kout, (const unsigned*)pin, pout, uk, 0, X.h + 1, st));
-        k_upd_flags<<<g, kUpdBlock, 0, st>>>(kout, k, n, flag);
-        CPB_CUDA(cudaGetLastError());
-        tb = tmp_b;
-        CPB_CUDA(cub::DeviceScan::ExclusiveSum(b + o_tmp, tb, (const unsigned*)flag, scan, uk, st));
-        k_upd_compact<<<g, kUpdBlock, 0, st>>>(kout, pout, flag, scan, k, X.h, digests, (u64*)(b + o_U), (u64*)(b + o_m),
-                                                scratch + 8 * X.off[X.h]);
-        CPB_CUDA(cudaGetLastError());
+        u32* scratch = B.scratch();
+        CPB_TRY(upd_run_plan<8>(B, X, idx, n, digests, st));
         const int l_grid_end = lt >= 0 ? lt + 1 : 0;
         for (int l = X.h - 1; l >= l_grid_end; l--) CPB_TRY(launch_level(node, X, l, scratch, leaf_nodes, nodes, st));
         if (lt >= 0) {
-            unsigned* arr = (unsigned*)(b + o_arr);
+            unsigned* arr = (unsigned*)B.extra();
             CPB_CUDA(cudaMemsetAsync(arr, 0, 4 * n_arr + 4, st));
             CPB_TRY(launch_top(node, X, lt, scratch, leaf_nodes, nodes, arr, st));
         }
-        k_upd_commit<<<upd_grid(X.off[X.h + 1], kUpdBlock), kUpdBlock, 0, st>>>(X, scratch, leaf_nodes, nodes, asserted, applied);
+        k_upd_commit<8><<<upd_grid(X.off[X.h + 1], kUpdBlock), kUpdBlock, 0, st>>>(X, scratch, leaf_nodes, nodes, asserted, applied);
         CPB_CUDA(cudaGetLastError());
         return CPB_OK;
     };
     const cpb_status rc = run();
-    cudaFreeAsync(b, st);
+    cudaFreeAsync(B.b, st);
     return rc;
 }
 
-// Shape rules shared by all four entry points, checked before any context or pointer is used.
-cpb_status check_update_shape(size_t n, size_t k) {
-    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
-    if (k >= ((size_t)1 << 32)) return fail(CPB_BAD_LENGTH, "an update holds fewer than 2^32 leaves (got %zu)", k);
-    return CPB_OK;
-}
 cpb_status check_update_ctxs(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node) {
     if (leaf) CPB_TRY(check_ctx(leaf));
     CPB_TRY(check_ctx(node));
@@ -383,8 +260,7 @@ cpb_status check_dev_args(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, uint64
     return check_update_ctxs(leaf, node);
 }
 
-// Host arrays: only the siblings the touched nodes read go up, only the touched nodes come back.  The device mirror of the tree
-// (node->s_aux, 2n - 1 elements: leaves, then inner nodes) is allocated but never filled beyond those siblings.
+// Host arrays: upd_host_form (merkle_update_kernels.cuh) around the _dev form.
 cpb_status update_host(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes, size_t n,
                        const uint64_t* indexes, const uint64_t* in, size_t leaf_len, size_t k, const uint64_t* asserted_root, int* applied) {
     const size_t in_elems = leaf ? leaf_len : 1;
@@ -397,57 +273,11 @@ cpb_status update_host(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, uint64_t*
         if (applied) *applied = !asserted_root || memcmp(non_leaf_nodes, asserted_root, 32) == 0;
         return CPB_OK;
     }
-    const int h = log2_exact(n);
-    std::vector<u64> uniq(indexes, indexes + k), reads, writes;
-    std::sort(uniq.begin(), uniq.end());
-    uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
-    upd_host_sets(uniq, h, reads, writes);
-    auto host_elem = [&](u64 pos) -> const uint64_t* { return pos < n ? leaf_nodes + 4 * pos : non_leaf_nodes + 4 * (pos - n); };
-    std::vector<uint64_t> read_vals(4 * reads.size());
-    for (size_t i = 0; i < reads.size(); i++) memcpy(&read_vals[4 * i], host_elem(reads[i]), 32);
-
-    std::lock_guard<std::mutex> lk(node->mu);
-    DeviceGuard g(node->device);
-    cudaStream_t st = node->stream;
-    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t b_in = 32 * k * in_elems, nr = reads.size(), nw = writes.size();
-    size_t o = 0;
-    const size_t o_idx = o; o += up(8 * k);
-    const size_t o_in = o; o += up(b_in ? b_in : 32);
-    const size_t o_root = o; o += 256;
-    const size_t o_rpos = o; o += up(8 * nr + 8);
-    const size_t o_rval = o; o += up(32 * nr + 32);
-    const size_t o_wpos = o; o += up(8 * nw);
-    CPB_TRY(node->s_in.reserve(o));
-    CPB_TRY(node->s_out.reserve(32 * nw + 256));
-    CPB_TRY(node->s_aux.reserve(32 * (2 * n - 1)));
-    char* d = (char*)node->s_in.ptr;
-    u32* mirror = (u32*)node->s_aux.ptr;
-    u32* d_out = (u32*)node->s_out.ptr;
-    unsigned char* d_applied = (unsigned char*)node->s_out.ptr + 32 * nw;
-    CPB_CUDA(cudaMemcpyAsync(d + o_idx, indexes, 8 * k, cudaMemcpyHostToDevice, st));
-    if (b_in) CPB_CUDA(cudaMemcpyAsync(d + o_in, in, b_in, cudaMemcpyHostToDevice, st));
-    if (asserted_root) CPB_CUDA(cudaMemcpyAsync(d + o_root, asserted_root, 32, cudaMemcpyHostToDevice, st));
-    if (nr) {
-        CPB_CUDA(cudaMemcpyAsync(d + o_rpos, reads.data(), 8 * nr, cudaMemcpyHostToDevice, st));
-        CPB_CUDA(cudaMemcpyAsync(d + o_rval, read_vals.data(), 32 * nr, cudaMemcpyHostToDevice, st));
-        k_upd_move<<<upd_grid(nr, kUpdBlock), kUpdBlock, 0, st>>>((const u32*)(d + o_rval), mirror, (const u64*)(d + o_rpos), nr, 0);
-        CPB_CUDA(cudaGetLastError());
-    }
-    CPB_CUDA(cudaMemcpyAsync(d + o_wpos, writes.data(), 8 * nw, cudaMemcpyHostToDevice, st));
-    CPB_TRY(update_dev(leaf, node, (uint64_t*)mirror, (uint64_t*)(mirror + 8 * n), n, (const uint64_t*)(d + o_idx), (const uint64_t*)(d + o_in),
-                       leaf_len, k, asserted_root ? (const uint64_t*)(d + o_root) : nullptr, d_applied, st));
-    k_upd_move<<<upd_grid(nw, kUpdBlock), kUpdBlock, 0, st>>>(mirror, d_out, (const u64*)(d + o_wpos), nw, 1);
-    CPB_CUDA(cudaGetLastError());
-    std::vector<uint64_t> write_vals(4 * nw);
-    unsigned char ok = 0;
-    CPB_CUDA(cudaMemcpyAsync(write_vals.data(), d_out, 32 * nw, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaMemcpyAsync(&ok, d_applied, 1, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    if (ok)
-        for (size_t i = 0; i < nw; i++) memcpy((void*)host_elem(writes[i]), &write_vals[4 * i], 32);
-    if (applied) *applied = ok;
-    return CPB_OK;
+    return upd_host_form<8>(node, leaf_nodes, non_leaf_nodes, n, indexes, in, 32 * k * in_elems, k, asserted_root, applied,
+                            [&](uint64_t* ml, uint64_t* mn, const uint64_t* d_idx, const void* d_in, const uint64_t* d_root, uint8_t* d_applied,
+                                cudaStream_t st) {
+                                return update_dev(leaf, node, ml, mn, n, d_idx, (const uint64_t*)d_in, leaf_len, k, d_root, d_applied, st);
+                            });
 }
 
 }  // namespace

@@ -16,6 +16,7 @@
 #include "common.cuh"
 #include "hostfp.hpp"
 #include "pedersen.cuh"
+#include "pedersen_internal.cuh"
 
 namespace cpb {
 
@@ -27,13 +28,6 @@ constexpr unsigned kChunkBytes = kChunkWords * 4;
 #define CPB_PEDERSEN_CHUNK_BITS 8
 #endif
 constexpr int kDefaultChunkBits = CPB_PEDERSEN_CHUNK_BITS;
-
-struct PedersenDev {
-    int chunk_bits;      // 8: shared-memory (TMA-staged) tables; 9..16: L2 / HBM resident tables, gathered per lookup
-    int n_in_chunks;     // ceil(input bits that can be set / chunk_bits); with 8-bit chunks = input bytes
-    int n_rand_chunks;   // ceil(#randomness generators / chunk_bits), 0 without commitment parameters
-    int zero;            // always 0 (see PoseidonDev::zero)
-};
 
 // consts layout (u32 words): [0..8) modulus limbs, [8..16) 2d (Montgomery), [16..24) d (Montgomery)
 template <class F>
@@ -496,18 +490,6 @@ __global__ void k_bh_children_to_bytes(const u32* __restrict__ children, uint8_t
 
 using namespace cpb;
 
-struct cpb_pedersen_ctx {
-    int curve_id = 0, field_id = 0, device = 0, sms = 132;
-    int window_size = 0, num_windows = 0, n_rand = 0;
-    size_t nbits = 0;
-    PedersenDev dev{};
-    u32* d_consts = nullptr;
-    u32* d_table = nullptr;
-    cudaStream_t stream = nullptr;
-    std::mutex mu;
-    Scratch s_in, s_out, s_aux, s_rand;
-};
-
 extern "C" cpb_status cpb_pedersen_ctx_create_ex(int, int, int, const uint64_t*, size_t, const uint64_t*, int, int, cpb_pedersen_ctx**);
 extern "C" int cpb_poseidon_ctx_field(const cpb_poseidon_ctx* ctx);
 extern "C" int cpb_poseidon_ctx_device(const cpb_poseidon_ctx* ctx);
@@ -545,6 +527,10 @@ template <class K> cpb_status ped_grid(K kernel, size_t smem, int sms, long n, i
     return CPB_OK;
 }
 
+}  // namespace
+
+namespace cpb {
+
 template <class F>
 cpb_status launch_hash_f(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, size_t stride, const uint8_t* rand32,
                          u32* out, size_t n, int mode, cudaStream_t st) {
@@ -570,7 +556,6 @@ cpb_status launch_hash_f(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, siz
     return CPB_OK;
 }
 
-// length rules of the reference: R/crh/pedersen/mod.rs:82-89 (CRH) and R/commitment/pedersen/mod.rs:69-71
 cpb_status check_len(const cpb_pedersen_ctx* c, size_t len, bool commit) {
     if (commit && len > c->nbits) return fail(CPB_BAD_LENGTH, "incorrect input length: %zu", len);
     if (len * 8 > c->nbits)
@@ -589,6 +574,15 @@ cpb_status launch_hash(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, size_
     return fail(CPB_UNSUPPORTED, "no kernel for base field %d", c->field_id);
 }
 
+size_t two_to_one_len(const cpb_pedersen_ctx* c) {
+    size_t half = c->nbits / 2, buf = (half + half) / 8;
+    return buf < 128 ? buf : 128;
+}
+
+}  // namespace cpb
+
+namespace {
+
 cpb_status launch_points_to_bytes(cpb_pedersen_ctx* c, const u32* children, u32* bytes, size_t n_nodes, cudaStream_t st) {
     long elems = (long)n_nodes * 4;
     int grid = (int)((elems + 255) / 256);
@@ -599,12 +593,6 @@ cpb_status launch_points_to_bytes(cpb_pedersen_ctx* c, const u32* children, u32*
     }
     CPB_CUDA(cudaGetLastError());
     return CPB_OK;
-}
-
-// TwoToOneCRH::evaluate buffer length, R/crh/pedersen/mod.rs:171: (HALF + HALF) / 8 with HALF = bits / 2
-size_t two_to_one_len(const cpb_pedersen_ctx* c) {
-    size_t half = c->nbits / 2, buf = (half + half) / 8;
-    return buf < 128 ? buf : 128;     // left||right of two 64-byte points; a longer buffer is zero padding
 }
 
 cpb_status two_to_one_dev(cpb_pedersen_ctx* c, const u32* children, u32* out, size_t n, u32* scratch_bytes, cudaStream_t st) {

@@ -91,6 +91,15 @@ CPB_HD UpdKids upd_kids(const u64* U, u64 m, int h, int l, u64 k, const UpdSite&
     return K;
 }
 
+// Where the current value of child `node` (level l + 1) of a touched node of level l is, for digests of W words: the scratch when
+// the child is touched too, the caller's tree otherwise (its leaf array below level h - 1, its heap-ordered inner nodes above).
+template <int W, class T>
+CPB_HD T* upd_child_at(const UpdPlan& X, int l, bool touched, u64 slot, u64 node, T* scratch, T* leaf_nodes, T* nodes) {
+    if (touched) return scratch + W * (X.off[l + 1] + slot);
+    if (l + 1 == X.h) return leaf_nodes + W * node;
+    return nodes + W * (((1ull << (l + 1)) - 1) + node);
+}
+
 // The candidate of level l - 1 that is the parent of node p of level l (l > 0).
 CPB_HD u64 upd_parent_cand(const u64* U, u64 m, int h, int l, u64 k, u64 p) {
     const u64 q = p >> 1;

@@ -74,4 +74,45 @@ template <class F> CPB_HD bool te_on_curve(const u32* x, const u32* y, const u32
     return fp_eq(l, r);
 }
 
+// Table index of lookup c of a `len`-byte message at `cb` bits per lookup (cb <= 22): bits [c cb, (c + 1) cb) of the message,
+// zero beyond len, little-endian -- up to four bytes, the value k_pedersen_hash_gather computes (for cb = 8, byte c).
+CPB_HD u32 te_lookup_value(const uint8_t* msg, long len, int c, int cb) {
+    const long bit = (long)c * cb, byte = bit >> 3;
+    u64 v = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        if (byte + k < len) v |= (u64)msg[byte + k] << (8 * k);
+    return (u32)(v >> (bit & 7)) & ((1u << cb) - 1u);
+}
+
+// One lane's share of a hash split over `lanes` lanes: the mixed additions of lookups c = lane, lane + lanes, ... < n_chunks, from
+// the identity.  entry(c, value, yp, ym, t2d) fetches the table entry.  The lanes' sums are then added in any order (the group is
+// abelian): the warp kernel of the Pedersen-node update (cpb_merkle_update_pedersen.cu) reduces them with shuffles and te_add.
+template <class F, class Entry>
+CPB_HD void te_lane_sum(TePoint& acc, const uint8_t* msg, long len, int cb, int n_chunks, int lane, int lanes, Entry&& entry, const u32* pm) {
+    te_identity<F>(acc);
+#pragma unroll 1
+    for (int c = lane; c < n_chunks; c += lanes) {
+        u32 yp[8], ym[8], t2d[8];
+        entry(c, te_lookup_value(msg, len, c, cb), yp, ym, t2d);
+        te_madd<F>(acc, yp, ym, t2d, pm);
+    }
+}
+
+// TwoToOneCRH::compress input of one node (R/crh/pedersen/mod.rs:187-197): the two children (affine x, y in Montgomery form)
+// serialised uncompressed -- canonical little-endian x_l || y_l || x_r || y_r, 32 words.  The same bytes as k_points_to_bytes
+// (cpb_pedersen.cu) writes for the build.
+template <class F> CPB_HD void te_node_row(u32* row, const u32* left, const u32* right) {
+    u32 pm[8], one[8], a[8];
+    fp_modulus<F>(pm);
+    fp_zero(one);
+    one[0] = 1;
+#pragma unroll 1
+    for (int j = 0; j < 4; j++) {
+        ld_elem(a, (j < 2 ? left : right) + 8 * (j & 1));
+        fp_mul<F>(a, a, one, pm);
+        st_elem(row + 8 * j, a);
+    }
+}
+
 }  // namespace cpb

@@ -211,6 +211,64 @@ class CudaMixedBackend(CudaPoseidonBackend):
         return self._update_digests(leaf_nodes, nodes, idx, digests, root, applied)
 
 
+class CudaPedersenBackend(CudaPoseidonBackend):
+    """Byte tree of JubJubMerkleTreeParams (R/merkle_tree/tests/mod.rs:19-33): byte leaves hashed with pedersen::CRH, inner nodes
+    with pedersen::TwoToOneCRH.  Digests are affine points, (2, 4) words; leaves: (n, leaf_len) uint8 on the GPU.  There is no
+    sharded build for byte trees."""
+
+    digest_words = 8
+
+    def __init__(self, leaf_params, node_params, device_index: int):
+        from . import _native as N
+        self.N = N
+        self.dev = device_index
+        self.leaf_ctx = leaf_params.context(device_index)
+        self.node_ctx = node_params.context(device_index)
+        self._ws = {}
+
+    def build_local(self, leaves: torch.Tensor):
+        """leaves (n, leaf_len) uint8 -> (leaf_nodes (n, 2, 4), nodes (n-1, 2, 4)) heap order."""
+        n, ln = leaves.shape
+        leaf_nodes = self._buf("leaf", (n, 2, 4), leaves.device)
+        nodes = self._buf("nodes", (n - 1, 2, 4), leaves.device)
+        scratch = self._buf("scratch", (n, 8), leaves.device)            # 64 bytes per leaf
+        self.N.check(self.N.lib.cpb_merkle_pedersen_build_dev(self.leaf_ctx, self.node_ctx, leaves.data_ptr(), ln, leaves.stride(0), n,
+                                                              leaf_nodes.data_ptr(), nodes.data_ptr(), scratch.data_ptr(), self._stream()))
+        return leaf_nodes, nodes
+
+    def build_sharded(self, leaves, ex):
+        raise NotImplementedError("byte trees have no sharded build")
+
+    def hash_leaves(self, leaves: torch.Tensor):
+        n, ln = leaves.shape
+        out = self._buf("leaf", (n, 2, 4), leaves.device)
+        self.N.check(self.N.lib.cpb_pedersen_crh_batch_dev(self.leaf_ctx, leaves.data_ptr(), ln, leaves.stride(0), out.data_ptr(), n,
+                                                           self._stream()))
+        return out
+
+    def from_digests(self, digests):
+        raise NotImplementedError("use build_local")
+
+    def update(self, leaf_nodes: torch.Tensor, nodes: torch.Tensor, indexes: torch.Tensor, new_leaves: torch.Tensor, asserted_root=None):
+        """k x MerkleTree::update -- or check_update when `asserted_root` (2, 4) is given -- on a tree built on this device, in place
+        and on the current stream: leaf_nodes (n, 2, 4), nodes (n-1, 2, 4) heap order, indexes (k,) (the last occurrence of a repeated
+        index wins; an index >= n is skipped), new_leaves (k, leaf_len) uint8, rows any stride apart.  Returns the device flag
+        `applied` (uint8, (1,)); no synchronisation."""
+        n = leaf_nodes.shape[0]
+        assert leaf_nodes.is_contiguous() and nodes.is_contiguous() and tuple(nodes.shape[1:]) == (2, 4) and nodes.shape[0] == n - 1
+        assert tuple(leaf_nodes.shape[1:]) == (2, 4)
+        idx = indexes.to(device=leaf_nodes.device, dtype=torch.int64).contiguous()
+        root = None if asserted_root is None else asserted_root.to(device=leaf_nodes.device, dtype=torch.int64).contiguous().clone()
+        applied = torch.empty(1, dtype=torch.uint8, device=leaf_nodes.device)
+        k, ln = new_leaves.shape
+        assert idx.shape[0] == k, "one new leaf per index"
+        assert new_leaves.dtype == torch.uint8 and (k == 0 or new_leaves.stride(1) == 1)
+        self.N.check(self.N.lib.cpb_merkle_pedersen_update_dev(self.leaf_ctx, self.node_ctx, leaf_nodes.data_ptr(), nodes.data_ptr(), n,
+                                                               idx.data_ptr(), new_leaves.data_ptr(), ln, new_leaves.stride(0), k,
+                                                               None if root is None else root.data_ptr(), applied.data_ptr(), self._stream()))
+        return applied
+
+
 @dataclass
 class ShardedTree:
     """Result of a sharded build on this rank."""

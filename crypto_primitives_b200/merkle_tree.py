@@ -10,7 +10,8 @@ mod.rs:547-623.  Verification and update are LEVEL-SYNCHRONOUS device batches fo
 leaves cost height launches, not k * height (`verify_paths_batch`, `MultiPath.verify`, `update_batch`);
 the Poseidon field-leaf Config additionally has a single-launch kernel that recomputes one root per
 thread (`cpb_merkle_poseidon_verify_batch`), and Configs whose inner hash is Poseidon update in ONE library
-call (`cpb_merkle_poseidon_update_digests`: every level on the device, only touched nodes cross PCIe).
+call (`cpb_merkle_poseidon_update_digests`, and `cpb_merkle_pedersen_update` for the Pedersen byte tree: every level on the
+device, only touched nodes cross PCIe).
 """
 from __future__ import annotations
 
@@ -474,13 +475,16 @@ class MerkleTree:
         return idx
 
     def _updates_on_device(self) -> bool:
-        """Configs whose inner hash is poseidon::TwoToOneCRH update through cpb_merkle_poseidon_update_digests: the touched nodes
-        of every level are hashed on the device in one call, and only they and the siblings they read cross PCIe."""
-        return type(self.config) in (PoseidonFieldConfig, PedersenPoseidonConfig)
+        """Configs whose inner hash is poseidon::TwoToOneCRH update through cpb_merkle_poseidon_update_digests, the Pedersen byte tree
+        through cpb_merkle_pedersen_update: the touched nodes of every level are hashed on the device in one call, and only they and
+        the siblings they read cross PCIe."""
+        return type(self.config) in (PoseidonFieldConfig, PedersenPoseidonConfig, PedersenByteConfig)
 
     def _update_digests(self, idx, new_leaves, asserted_new_root=None) -> bool:
         """The Config's leaf hash of `new_leaves`, then one update call on the tree's arrays in place; True when applied."""
         cfg, dev = self.config, self.device
+        if type(cfg) is PedersenByteConfig:
+            return self._update_pedersen(idx, new_leaves, asserted_new_root)
         new_hash = np.ascontiguousarray(cfg.leaf_hash_batch(self.leaf_hash_param, _leaf_batch(new_leaves), dev), dtype=np.uint64).reshape(-1, 4)
         assert new_hash.shape[0] == idx.size, "one new leaf per index"
         self.leaf_nodes = np.ascontiguousarray(self.leaf_nodes, dtype=np.uint64)
@@ -493,11 +497,32 @@ class MerkleTree:
                                                          None if root is None else _p(root), C.byref(ok)))
         return bool(ok.value)
 
+    def _update_pedersen(self, idx, new_leaves, asserted_new_root=None) -> bool:
+        """Byte tree with Pedersen inner nodes: the byte leaves and the indexes go to cpb_merkle_pedersen_update, which hashes the
+        leaves and every touched node on the device in one call."""
+        lv = np.ascontiguousarray(new_leaves, dtype=np.uint8)
+        assert lv.ndim == 2 and lv.shape[0] == idx.size, "one new leaf (bytes) per index"
+        self.leaf_nodes = np.ascontiguousarray(self.leaf_nodes, dtype=np.uint64)
+        self.non_leaf_nodes = np.ascontiguousarray(self.non_leaf_nodes, dtype=np.uint64)
+        ix = np.ascontiguousarray(idx, dtype=np.uint64)
+        root = None if asserted_new_root is None else np.ascontiguousarray(asserted_new_root, dtype=np.uint64).reshape(8)
+        ok = C.c_int(0)
+        try:
+            N.check(N.lib.cpb_merkle_pedersen_update(self.leaf_hash_param.context(self.device), self.two_to_one_hash_param.context(self.device),
+                                                     _p(self.leaf_nodes), _p(self.non_leaf_nodes), self.leaf_nodes.shape[0], _p(ix),
+                                                     lv.ctypes.data_as(N.u8p), lv.shape[1], ix.size, None if root is None else _p(root),
+                                                     C.byref(ok)))
+        except N.CpbError as e:
+            if e.status == N.CPB_BAD_LENGTH:
+                raise ValueError("incorrect input length") from e
+            raise
+        return bool(ok.value)
+
     def _updated_nodes(self, indexes, new_leaves):
         """The nodes that change when leaves `indexes` (distinct) are replaced by `new_leaves` (mod.rs:627-677 for one leaf):
         -> (new leaf digests, [(heap indexes, new values)] bottom level first).  Level-synchronous: the new leaves are one
         leaf-hash batch and all touched nodes of a level one two-to-one batch -- height launches for any number of leaves.
-        The path of Configs without a Poseidon inner hash (Pedersen / Bowe-Hopwood nodes, toy Configs)."""
+        The path of the Configs without a one-call device update (Bowe-Hopwood nodes, toy Configs)."""
         cfg, dev = self.config, self.device
         idx = self._check_indexes(indexes)
         n = self.leaf_nodes.shape[0]

@@ -328,6 +328,36 @@ cpb_status cpb_merkle_pedersen_build(cpb_pedersen_ctx* leaf_ctx, cpb_pedersen_ct
 cpb_status cpb_merkle_pedersen_build_dev(cpb_pedersen_ctx* leaf_ctx, cpb_pedersen_ctx* node_ctx, const uint8_t* leaves,
                                          size_t leaf_len, size_t leaf_stride, size_t n, uint64_t* leaf_nodes_xy,
                                          uint64_t* non_leaf_nodes_xy, void* scratch_64n, void* stream);
+
+/* ---- Merkle tree update (Pedersen inner nodes) ------------------------------------------------------------------ */
+/* k x MerkleTree::update / check_update on a byte tree of cpb_merkle_pedersen_build (inner hash pedersen::TwoToOneCRH), with the
+ * rules of cpb_merkle_poseidon_update* word for word: the result equals k sequential updates in input order (the last occurrence
+ * of a repeated index wins); with asserted_root_xy (8 words) nothing is written unless the new root matches, and `applied` says
+ * which happened; k == 0 is a no-op whose `applied` says whether the current root equals asserted_root_xy; n not a power of two
+ * > 1 -> CPB_NOT_POW2; k >= 2^32 -> CPB_BAD_LENGTH before any array is read; _dev forms skip an index >= n, host forms return
+ * CPB_BAD_PARAMS for it before any copy.  Digests are affine points (8 words each, as the build writes them).
+ * The digest forms take new_leaf_digests_xy[k] (e.g. cpb_pedersen_crh_batch outputs); the leaf forms take byte leaves and hash
+ * all k of them with leaf_ctx on the same stream first: leaf i at new_leaves + i * leaf_stride (_dev form) or packed k x leaf_len
+ * (host form); leaf_len * 8 > WINDOW_SIZE * NUM_WINDOWS of leaf_ctx -> CPB_BAD_LENGTH, as the CRH; leaf_stride < leaf_len with
+ * k > 1 -> CPB_BAD_PARAMS.  Both curves and every chunk
+ * width of cpb_pedersen_ctx_create_ex.
+ * _dev forms: device pointers, no host synchronisation, scratch from the stream-ordered pool (about sum over levels l of
+ * min(k, 2^l) points plus 128 bytes per slot of the widest inner level); launches depend on the tree height only -- per wide inner
+ * level one row kernel and the node context's hash and normalisation, then one warp-per-node launch for the narrow levels above.  Host forms: host arrays; only the siblings the touched
+ * nodes read are uploaded and only the touched nodes come back. */
+cpb_status cpb_merkle_pedersen_update_digests_dev(cpb_pedersen_ctx* node_ctx, uint64_t* leaf_nodes_xy, uint64_t* non_leaf_nodes_xy, size_t n,
+                                                  const uint64_t* indexes, const uint64_t* new_leaf_digests_xy, size_t k,
+                                                  const uint64_t* asserted_root_xy, uint8_t* applied, void* stream);
+cpb_status cpb_merkle_pedersen_update_dev(cpb_pedersen_ctx* leaf_ctx, cpb_pedersen_ctx* node_ctx, uint64_t* leaf_nodes_xy,
+                                          uint64_t* non_leaf_nodes_xy, size_t n, const uint64_t* indexes, const uint8_t* new_leaves,
+                                          size_t leaf_len, size_t leaf_stride, size_t k, const uint64_t* asserted_root_xy, uint8_t* applied,
+                                          void* stream);
+cpb_status cpb_merkle_pedersen_update_digests(cpb_pedersen_ctx* node_ctx, uint64_t* leaf_nodes_xy, uint64_t* non_leaf_nodes_xy, size_t n,
+                                              const uint64_t* indexes, const uint64_t* new_leaf_digests_xy, size_t k,
+                                              const uint64_t* asserted_root_xy, int* applied);
+cpb_status cpb_merkle_pedersen_update(cpb_pedersen_ctx* leaf_ctx, cpb_pedersen_ctx* node_ctx, uint64_t* leaf_nodes_xy, uint64_t* non_leaf_nodes_xy,
+                                      size_t n, const uint64_t* indexes, const uint8_t* new_leaves, size_t leaf_len, size_t k,
+                                      const uint64_t* asserted_root_xy, int* applied);
 /* MerkleTree::new for Config{Leaf=[u8], LeafHash=PedersenCRHCompressor<C,TECompressor,W>,
  * IdentityDigestConverter, TwoToOneHash=poseidon::TwoToOneCRH<Fq>} (BASELINE config 5): leaf digest =
  * x-coordinate, a base-field element; the Poseidon field must be the curve's base field. */

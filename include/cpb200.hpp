@@ -185,6 +185,62 @@ struct Commitment {   // R/commitment/pedersen/mod.rs:38-106; randomness = 32-by
 
 }  // namespace pedersen
 
+// MerkleTree of JubJubMerkleTreeParams (R/merkle_tree/tests/mod.rs:19-33): byte leaves, pedersen::CRH leaf hash, ByteDigestConverter,
+// pedersen::TwoToOneCRH inner nodes.  Digests are affine points.
+class PedersenMerkleTree {
+public:
+    std::vector<Affine> leaf_nodes, non_leaf_nodes;   // the reference's two arrays (mod.rs:383-395)
+
+    // n leaves of leaf_len bytes each, back to back
+    static PedersenMerkleTree create(const pedersen::Parameters& leaf, const pedersen::Parameters& two_to_one, const std::vector<uint8_t>& leaves,
+                                     size_t leaf_len) {
+        PedersenMerkleTree t;
+        const size_t n = leaf_len ? leaves.size() / leaf_len : 0;
+        t.leaf_nodes.resize(n);
+        t.non_leaf_nodes.resize(n ? n - 1 : 0);
+        check(cpb_merkle_pedersen_build(leaf.ctx(), two_to_one.ctx(), leaves.empty() ? nullptr : leaves.data(), leaf_len, n,
+                                        n ? t.leaf_nodes[0].x.data() : nullptr, n > 1 ? t.non_leaf_nodes[0].x.data() : nullptr));
+        return t;
+    }
+    Affine root() const { return non_leaf_nodes.at(0); }
+    size_t height() const {
+        size_t h = 1, n = leaf_nodes.size();
+        while (n > 1) { n >>= 1; h++; }
+        return h;
+    }
+
+    // k x MerkleTree::update (mod.rs:690-701) in one call: leaf indexes[i] becomes leaves[i * leaf_len .. (i+1) * leaf_len) (bytes); a
+    // repeated index takes its last leaf.  Only the touched nodes and the siblings they read cross PCIe.
+    void update_batch(const pedersen::Parameters& leaf, const pedersen::Parameters& two_to_one, const std::vector<uint64_t>& indexes,
+                      const std::vector<uint8_t>& leaves, size_t leaf_len) {
+        update_impl(leaf, two_to_one, indexes, leaves, leaf_len, nullptr);
+    }
+    void update(const pedersen::Parameters& leaf, const pedersen::Parameters& two_to_one, size_t index, const std::vector<uint8_t>& new_leaf) {
+        update_batch(leaf, two_to_one, {(uint64_t)index}, new_leaf, new_leaf.size());
+    }
+    // check_update (mod.rs:706-725) for all k at once: the tree changes only when the new root equals asserted_new_root.
+    bool check_update_batch(const pedersen::Parameters& leaf, const pedersen::Parameters& two_to_one, const std::vector<uint64_t>& indexes,
+                            const std::vector<uint8_t>& leaves, size_t leaf_len, const Affine& asserted_new_root) {
+        return update_impl(leaf, two_to_one, indexes, leaves, leaf_len, &asserted_new_root);
+    }
+    bool check_update(const pedersen::Parameters& leaf, const pedersen::Parameters& two_to_one, size_t index, const std::vector<uint8_t>& new_leaf,
+                      const Affine& asserted_new_root) {
+        return check_update_batch(leaf, two_to_one, {(uint64_t)index}, new_leaf, new_leaf.size(), asserted_new_root);
+    }
+
+private:
+    bool update_impl(const pedersen::Parameters& leaf, const pedersen::Parameters& two_to_one, const std::vector<uint64_t>& indexes,
+                     const std::vector<uint8_t>& leaves, size_t leaf_len, const Affine* asserted) {
+        const size_t k = indexes.size();
+        if (leaves.size() != k * leaf_len) throw Error(CPB_BAD_LENGTH, "one leaf of leaf_len bytes per index");
+        int applied = 0;
+        check(cpb_merkle_pedersen_update(leaf.ctx(), two_to_one.ctx(), leaf_nodes.empty() ? nullptr : leaf_nodes[0].x.data(),
+                                         non_leaf_nodes.empty() ? nullptr : non_leaf_nodes[0].x.data(), leaf_nodes.size(), indexes.data(),
+                                         leaves.empty() ? nullptr : leaves.data(), leaf_len, k, asserted ? asserted->x.data() : nullptr, &applied));
+        return applied != 0;
+    }
+};
+
 // Byte strings of different lengths as the C-ABI's ragged batch: the bytes back to back plus n + 1 offsets.
 inline void ragged_pack(const std::vector<std::vector<uint8_t>>& inputs, std::vector<uint8_t>& values, std::vector<uint64_t>& offsets) {
     offsets.assign(1, 0);

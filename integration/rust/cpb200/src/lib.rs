@@ -339,6 +339,12 @@ pub mod pedersen {
         fn cpb_pedersen_crh_batch(ctx: *mut cpb_pedersen_ctx, input: *const u8, len: usize, stride: usize, out_xy: *mut u64, n: usize) -> c_int;
         fn cpb_pedersen_commit_batch(ctx: *mut cpb_pedersen_ctx, input: *const u8, len: usize, stride: usize, randomness_le32: *const u8,
                                      out_xy: *mut u64, n: usize) -> c_int;
+        fn cpb_merkle_pedersen_build(leaf: *mut cpb_pedersen_ctx, node: *mut cpb_pedersen_ctx, leaves: *const u8, leaf_len: usize, n: usize,
+                                     leaf_nodes_xy: *mut u64, non_leaf_nodes_xy: *mut u64) -> c_int;
+        // k x MerkleTree::update / check_update of a byte tree on host arrays in place; asserted_root_xy and applied may be null
+        fn cpb_merkle_pedersen_update(leaf: *mut cpb_pedersen_ctx, node: *mut cpb_pedersen_ctx, leaf_nodes_xy: *mut u64,
+                                      non_leaf_nodes_xy: *mut u64, n: usize, indexes: *const u64, new_leaves: *const u8, leaf_len: usize,
+                                      k: usize, asserted_root_xy: *const u64, applied: *mut c_int) -> c_int;
     }
 
     struct Ctx(*mut cpb_pedersen_ctx);
@@ -408,6 +414,74 @@ pub mod pedersen {
             let mut out = [0u64; 8];
             check(unsafe { cpb_pedersen_crh_batch(p.ctx.0, input.as_ptr(), input.len(), input.len(), out.as_mut_ptr(), 1) })?;
             Ok(points(&out)[0])
+        }
+    }
+
+    fn affine_limbs(points: &[EdwardsAffine]) -> Vec<u64> {
+        points.iter().flat_map(|p| [p.x.mont_limbs(), p.y.mont_limbs()].concat()).collect()
+    }
+
+    /// `MerkleTree<JubJubMerkleTreeParams>` (R/merkle_tree/tests/mod.rs:19-33: byte leaves, pedersen::CRH leaf hash,
+    /// ByteDigestConverter, pedersen::TwoToOneCRH inner nodes) built and updated on the GPU.  The ABI returns the reference's own two
+    /// arrays (R/merkle_tree/mod.rs:383-395) of affine points, so proofs are the reference's index arithmetic.
+    pub struct GpuPedersenMerkleTree {
+        pub leaf_nodes: Vec<EdwardsAffine>,
+        pub non_leaf_nodes: Vec<EdwardsAffine>,
+        height: usize,
+    }
+    impl GpuPedersenMerkleTree {
+        /// `MerkleTree::new` over leaves of one byte length (Pedersen zero-pads, R/crh/pedersen/mod.rs:94-99).
+        pub fn new(leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, leaves: &[Vec<u8>]) -> Result<Self, Error> {
+            let n = leaves.len();
+            let leaf_len = leaves.first().map_or(0, |l| l.len());
+            assert!(leaves.iter().all(|l| l.len() == leaf_len), "leaves of one length");
+            let flat: Vec<u8> = leaves.concat();
+            let (mut ln, mut nn) = (vec![0u64; 8 * n], vec![0u64; 8 * n.saturating_sub(1)]);
+            check(unsafe { cpb_merkle_pedersen_build(leaf.ctx.0, two_to_one.ctx.0, flat.as_ptr(), leaf_len, n, ln.as_mut_ptr(), nn.as_mut_ptr()) })?;
+            Ok(Self { leaf_nodes: points(&ln), non_leaf_nodes: points(&nn), height: n.trailing_zeros() as usize + 1 })
+        }
+        pub fn root(&self) -> EdwardsAffine { self.non_leaf_nodes[0] }
+        pub fn height(&self) -> usize { self.height }
+        /// k x `MerkleTree::update` (R/merkle_tree/mod.rs:690-701) in one call: the new leaves and the touched nodes of every level
+        /// are hashed on the GPU, and only those nodes and the siblings they read cross PCIe.  A repeated index takes its last leaf;
+        /// new leaves of one length.
+        pub fn update_batch(&mut self, leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, indexes: &[usize], new_leaves: &[Vec<u8>])
+                            -> Result<(), Error> {
+            self.update_impl(leaf, two_to_one, indexes, new_leaves, None).map(|_| ())
+        }
+        pub fn update(&mut self, leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, index: usize, new_leaf: &[u8]) -> Result<(), Error> {
+            self.update_batch(leaf, two_to_one, &[index], &[new_leaf.to_vec()])
+        }
+        /// `MerkleTree::check_update` (mod.rs:706-725) for all k at once: the tree changes only when the new root equals
+        /// `asserted_new_root`; returns whether it did.
+        pub fn check_update_batch(&mut self, leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, indexes: &[usize],
+                                  new_leaves: &[Vec<u8>], asserted_new_root: &EdwardsAffine) -> Result<bool, Error> {
+            self.update_impl(leaf, two_to_one, indexes, new_leaves, Some(asserted_new_root))
+        }
+        pub fn check_update(&mut self, leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, index: usize, new_leaf: &[u8],
+                            asserted_new_root: &EdwardsAffine) -> Result<bool, Error> {
+            self.check_update_batch(leaf, two_to_one, &[index], &[new_leaf.to_vec()], asserted_new_root)
+        }
+        fn update_impl(&mut self, leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, indexes: &[usize], new_leaves: &[Vec<u8>],
+                       asserted_new_root: Option<&EdwardsAffine>) -> Result<bool, Error> {
+            assert_eq!(indexes.len(), new_leaves.len(), "one new leaf per index");
+            let leaf_len = new_leaves.first().map_or(0, |l| l.len());
+            assert!(new_leaves.iter().all(|l| l.len() == leaf_len), "an update batch takes new leaves of one length");
+            let idx: Vec<u64> = indexes.iter().map(|&i| i as u64).collect();
+            let flat: Vec<u8> = new_leaves.concat();
+            let (mut ln, mut nn) = (affine_limbs(&self.leaf_nodes), affine_limbs(&self.non_leaf_nodes));
+            let root = asserted_new_root.map(|r| affine_limbs(&[*r]));
+            let mut applied: c_int = 0;
+            check(unsafe {
+                cpb_merkle_pedersen_update(leaf.ctx.0, two_to_one.ctx.0, ln.as_mut_ptr(), nn.as_mut_ptr(), self.leaf_nodes.len(), idx.as_ptr(),
+                                           flat.as_ptr(), leaf_len, idx.len(), root.as_ref().map_or(core::ptr::null(), |r| r.as_ptr()),
+                                           &mut applied)
+            })?;
+            if applied != 0 {
+                self.leaf_nodes = points(&ln);
+                self.non_leaf_nodes = points(&nn);
+            }
+            Ok(applied != 0)
         }
     }
 
