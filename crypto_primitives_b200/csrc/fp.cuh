@@ -255,9 +255,9 @@ template <class F> CPB_HD void first_row(u32* E, u32* O, const u32* a, u32 bi, c
     redc_row<F>(E, O, pm);
 }
 
-// Later rows.  On entry `O` is the previous row's even accumulator (low limb zero) and `E`
-// the previous odd one: V/2^32 = E + O[1] + 2^32 * (O >> 64).  Adds a*bi, then reduces.
-template <class F> CPB_HD void next_row(u32* E, u32* O, const u32* a, u32 bi, const u32* pm) {
+// V = V/2^32 + a*bi.  On entry `O` is the previous row's even accumulator, whose low limb is dropped (zero after a reduction
+// row, a finished limb of the product in fp_mul_wide), and `E` the previous odd one: V/2^32 = E + O[1] + 2^32 * (O >> 64).
+CPB_HD void shift_mul_row(u32* E, u32* O, const u32* a, u32 bi) {
     E[0] = add_cc(E[0], O[1]);
     madc_wide_cc_from(O[0], O[1], a[1], bi, O[2], O[3]);
     madc_wide_cc_from(O[2], O[3], a[3], bi, O[4], O[5]);
@@ -268,10 +268,40 @@ template <class F> CPB_HD void next_row(u32* E, u32* O, const u32* a, u32 bi, co
     madc_wide_cc(E[4], E[5], a[4], bi);
     madc_wide_cc(E[6], E[7], a[6], bi);
     O[7] = addc(O[7], 0);
+}
+
+// Later rows of the CIOS product: adds a*bi to the shifted value, then reduces.
+template <class F> CPB_HD void next_row(u32* E, u32* O, const u32* a, u32 bi, const u32* pm) {
+    shift_mul_row(E, O, a, bi);
     redc_row<F>(E, O, pm);
 }
 
 }  // namespace detail
+
+// T = a*b, all 512 bits (16 limbs, no reduction): the rows of fp_mul without their reduction rows, 64 wide multiply-adds.  Row i
+// finishes limb i of T (the low limb of its even accumulator); the last row's two accumulators hold limbs 7..15.  The running
+// value a*(b mod 2^(32(i+1)))/2^(32i) stays below 2^288, so the 9 limbs of (E, O) never carry out.
+CPB_HD void fp_mul_wide(u32 (&T)[16], const u32* a, const u32* b) {
+    u32 ev[8], od[8];
+#pragma unroll
+    for (int j = 0; j < 8; j += 2) {
+        mul_wide(ev[j], ev[j + 1], a[j], b[0]);
+        mul_wide(od[j], od[j + 1], a[j + 1], b[0]);
+    }
+    T[0] = ev[0];
+#pragma unroll
+    for (int i = 1; i < 8; i++) {
+        u32* Ea = (i & 1) ? od : ev;    // as fp_mul: the accumulators swap roles every row
+        u32* Oa = (i & 1) ? ev : od;
+        detail::shift_mul_row(Ea, Oa, a, b[i]);
+        T[i] = Ea[0];
+    }
+    // the last row used E = od, O = ev:  limbs 8.. = (od >> 32) + ev
+    T[8] = add_cc(ev[0], od[1]);
+#pragma unroll
+    for (int i = 1; i < 7; i++) T[8 + i] = addc_cc(ev[i], od[i + 1]);
+    T[15] = addc(ev[7], 0);
+}
 
 // r = a*b/R mod p, fully reduced.  a, b in [0,p).  r may alias a or b.
 // LAZY (fields with slack, see F::LAZY5): the conditional subtraction is skipped and r = (a*b + M*p)/R < p*(a*b/(R*p) + 1) is
@@ -684,12 +714,9 @@ template <class F> CPB_HD void fp_add_lazy(u32* r, const u32* a, const u32* b) {
 }
 
 
-// r = a*a/R mod p.  Dedicated squaring: the 28 cross products are computed once and doubled with
-// adds (the ALU pipe has slack, the multiply pipe does not), then the 8 diagonal squares are added
-// and the 512-bit value goes through 8 Montgomery reduction rows.  100 wide multiply-adds (84 for
-// BLS12-381 Fr) against 128 (112) for fp_mul(a, a).
-// LAZY: a < 2^256 with a^2 < R*p; the result (a^2 + M*p)/R < p*(a^2/(R*p) + 1) is returned without the conditional subtraction.
-template <class F, bool LAZY> CPB_HD void fp_sqr(u32* r, const u32* a, const u32* pm) {
+// T = a*a, all 512 bits (16 limbs, no reduction): the 28 cross products are computed once and doubled with adds (the ALU pipe has
+// slack, the multiply pipe does not), then the 8 diagonal squares are added.  36 wide multiply-adds.
+CPB_HD void fp_sqr_wide(u32 (&T)[16], const u32* a) {
     // Cross products a_i*a_j (i<j) sit at limb i+j.  Even positions accumulate in E (index = limb),
     // odd positions in O (index = limb-1), so every product is an aligned 64-bit multiply-add and each
     // row is one carry chain per array.  A chain's carry-out always lands on a limb no earlier row
@@ -736,7 +763,6 @@ template <class F, bool LAZY> CPB_HD void fp_sqr(u32* r, const u32* a, const u32
     // row 6
     mad_wide_end_from(O[12], O[13], a[6], a[7], O[12]);
     // T = E + (O << 32)        (E[0] = E[1] = 0, nothing above E[13] / O[13])
-    u32 T[16];
     T[0] = 0;
     T[1] = O[0];
     T[2] = add_cc(E[2], O[1]);
@@ -752,6 +778,14 @@ template <class F, bool LAZY> CPB_HD void fp_sqr(u32* r, const u32* a, const u32
     mad_wide_cc(T[0], T[1], a[0], a[0]);
 #pragma unroll
     for (int i = 1; i < 8; i++) madc_wide_cc(T[2 * i], T[2 * i + 1], a[i], a[i]);
+}
+
+// r = a*a/R mod p.  Dedicated squaring: fp_sqr_wide, then the 512-bit value goes through 8 Montgomery reduction rows.  100 wide
+// multiply-adds (84 for BLS12-381 Fr) against 128 (112) for fp_mul(a, a).
+// LAZY: a < 2^256 with a^2 < R*p; the result (a^2 + M*p)/R < p*(a^2/(R*p) + 1) is returned without the conditional subtraction.
+template <class F, bool LAZY> CPB_HD void fp_sqr(u32* r, const u32* a, const u32* pm) {
+    u32 T[16];
+    fp_sqr_wide(T, a);
     // Montgomery reduction of the 16-limb T with a rolling 9-limb window (ev, od) and no overflow word.  Limb i + 7 of T enters at
     // row i (i >= 1), limb 15 after the last row, so after row i the window holds (T mod 2^(32(i+8)) + M*p) / 2^(32i) with
     // M < 2^(32(i+1)): below 2^256 + 2^32*p < 2^288 for ANY a < 2^256 whenever p < 2^256 - 2^224 (every field tag).  The

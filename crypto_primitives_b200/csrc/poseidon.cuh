@@ -110,6 +110,22 @@ template <class F, bool LAZY> CPB_HD void pos_sbox5(u32* x, const u32* pm) {
     fp_mul<F, LAZY>(x, x2, x, pm);
 }
 
+// x^5 for the 32 hashes of a converged warp (pos_permute_split with TC): each product's 512 bits on the integer pipe (fp_sqr_wide,
+// fp_mul_wide), its Montgomery reduction on the tensor cores (tc_redc over the R^-1 table rinv, tcbuf the warp's buffer).  Not
+// reduced: every result is below T/R + p * (1 + 2^-19), which keeps the LAZY bounds of pos_permute_split (BN254 Fr: x < 2p gives
+// x^2 < 1.76p, x^4 < 1.59p, x^5 < 1.60p; a canonical x gives x^5 < 1.24p; tests/test_poseidon_tc_redc.py).
+template <class F> CPB_HD void pos_sbox5_tc(u32* x, const u32* rinv, u32* tcbuf, const u32* pm) {
+#if defined(__CUDA_ARCH__)
+    u32 T[16], x2[8];
+    fp_sqr_wide(T, x);
+    tc_redc<F>(x2, T, rinv, tcbuf, pm);
+    fp_sqr_wide(T, x2);
+    tc_redc<F>(x2, T, rinv, tcbuf, pm);
+    fp_mul_wide(T, x2, x);
+    tc_redc<F>(x, T, rinv, tcbuf, pm);
+#endif
+}
+
 // The permutation, one rolled loop over all RF+RP rounds with a single instance of each
 // arithmetic body:  [add round constants] -> S-box on T lanes or lane 0 -> linear layer as
 // lazy dot products (T rows of a dense matrix, or the one dense row of the sparse form
@@ -146,11 +162,12 @@ struct PermuteHint {
 // A5: the exponent is 5, known at compile time (P.alpha is not read).  Every S-box is then the straight-line pos_sbox5, with no
 // run-time exponent test and no generic square-and-multiply body in either loop.
 // TC (device only, BN254 Fr t = 3 with A5): the partial rounds' products by constants run on the tensor cores (tc_partial_round,
-// poseidon_tc.cuh) over P.tab8, with the same result ranges as the table path.  The whole warp must be converged and run the same
-// schedule; tcbuf is the warp's kTcWarpWords of shared memory.
+// poseidon_tc.cuh) over P.tab8, with the same result ranges as the table path, and every S-box reduces its products there
+// (pos_sbox5_tc over the R^-1 table tcrinv in shared memory).  The whole warp must be converged and run the same schedule; tcbuf
+// is the warp's kTcWarpWords of shared memory.
 template <class F, int T, bool A5 = false, bool TC = false>
 CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* cs, const u32* pm, const PermuteHint& H,
-                              u32* tcbuf = nullptr) {
+                              u32* tcbuf = nullptr, const u32* tcrinv = nullptr) {
     const int half = P.rf / 2;
     int top_bit = 0;
     if (!A5)
@@ -185,6 +202,7 @@ CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* c
 #pragma unroll 1
             for (int j = 0; j < T; j++) {
                 if (j == first_j) ld_elem(s[0], cs + 8 * P.off_sc0);         // S(0 + c) of the schedule
+                else if constexpr (TC) pos_sbox5_tc<F>(s[0], tcrinv, tcbuf, pm);
                 else if constexpr (A5) pos_sbox5<F, LZ>(s[0], pm);
                 else if (alpha_zero) fp_one<F>(s[0]);
                 else pos_sbox<F>(s[0], P.alpha, top_bit, pm, lazy);
@@ -245,7 +263,9 @@ CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* c
             const u32* trow = tk;
 #pragma unroll 1
             for (int k = 0; k < P.rp; k++, row += 8 * (2 * T - 2), trow += 64 * (2 * T - 2), pc += 8) {
-                if constexpr (A5) {
+                if constexpr (TC) {
+                    pos_sbox5_tc<F>(s[0], tcrinv, tcbuf, pm);
+                } else if constexpr (A5) {
                     pos_sbox5<F, LZ>(s[0], pm);
                 } else {
 #if CPB_SBOX5
@@ -319,10 +339,10 @@ CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* c
 // A5: see pos_permute_split; dense schedules take the merged loop, which reads P.alpha.
 template <class F, int T, bool A5 = false, bool TC = false>
 CPB_HD void pos_permute(u32 (&s)[T][8], const PoseidonDev& P, const u32* cs, const u32* pm, const PermuteHint& H = PermuteHint{0, ~0u},
-                        u32* tcbuf = nullptr) {
+                        u32* tcbuf = nullptr, const u32* tcrinv = nullptr) {
     if constexpr (CPB_POS_SPLIT_FOR(F)) {
         if (P.sparse) {
-            pos_permute_split<F, T, A5, TC>(s, P, cs, pm, H, tcbuf);
+            pos_permute_split<F, T, A5, TC>(s, P, cs, pm, H, tcbuf, tcrinv);
             return;
         }
     }
@@ -459,7 +479,7 @@ CPB_HD void pos_sponge(u32* out, long n_out, const u32* in, long len, const Pose
 // TC: see pos_permute_split; a lane with !live (past the end of the batch) hashes a zero input and stores nothing.
 template <class F, int T, bool A5 = false, bool TC = false>
 CPB_HD void pos_hash_single(u32* out, int n_out, const u32* in, int len, const PoseidonDev& P, const u32* cs, const u32* pm,
-                            u32* tcbuf = nullptr, bool live = true) {
+                            u32* tcbuf = nullptr, const u32* tcrinv = nullptr, bool live = true) {
     u32 s[T][8];
     const int cap = P.cap;
 #pragma unroll
@@ -468,7 +488,7 @@ CPB_HD void pos_hash_single(u32* out, int n_out, const u32* in, int len, const P
         if (live && lane >= 0 && lane < len) ld_elem(s[i], in + 8 * lane);
         else fp_zero(s[i]);
     }
-    pos_permute<F, T, A5, TC>(s, P, cs, pm, PermuteHint{1, ((1u << n_out) - 1u) << cap}, tcbuf);
+    pos_permute<F, T, A5, TC>(s, P, cs, pm, PermuteHint{1, ((1u << n_out) - 1u) << cap}, tcbuf, tcrinv);
 #pragma unroll
     for (int i = 0; i < T; i++) {
         const int lane = i - cap;

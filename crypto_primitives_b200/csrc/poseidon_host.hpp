@@ -382,31 +382,42 @@ inline PoseidonSchedule derive_schedule(const Field& F, const PoseidonParams& P,
     return S;
 }
 
-// Byte-digit tables of the tensor-core partial rounds (poseidon_tc.cuh), t = 3 sparse schedules: per partial round k the B
-// fragments of K8_i(c) = c * 2^(8i) * 2^32 / R mod p (i = 0..31) for c = gamma_k, alpha_k, beta_k, v_k (the lp region at
-// off_sc0 + 1), word tc_tab_word(nt, kc, lane, r) = bytes q = 0..3 of B[tc_b_k(lane, r, q)][8 nt + tc_b_col(lane)] of constant kc.
+// The B fragments of K8_i(c) = c * 2^(8i) * 2^32 / R mod p (i = 0..31) as constant kc of a table of `terms` constants at o: word
+// tc_tab_word(nt, kc, lane, r, terms) = bytes q = 0..3 of B[tc_b_k(lane, r, q)][8 nt + tc_b_col(lane)].
+inline void tc_put_table(const Field& F, const Fe& c, u32* o, int kc, int terms) {
+    unsigned char b[32][32];                              // [i][byte n] of K8_i(c)
+    Fe z{{1ull << 32, 0, 0, 0}};                          // 2^(8i + 32) mod p
+    for (int i = 0; i < 32; i++) {
+        const Fe v = F.mul(c, z);
+        for (int n = 0; n < 32; n++) b[i][n] = (unsigned char)(v.l[n / 8] >> (8 * (n % 8)));
+        for (int d = 0; d < 8; d++) z = F.add(z, z);
+    }
+    for (int nt = 0; nt < 4; nt++)
+        for (int lane = 0; lane < 32; lane++)
+            for (int r = 0; r < 2; r++) {
+                u32 w = 0;
+                for (int q = 0; q < 4; q++) w |= (u32)b[tc_b_k(lane, r, q)][8 * nt + tc_b_col(lane)] << (8 * q);
+                o[tc_tab_word(nt, kc, lane, r, terms)] = w;
+            }
+}
+
+// Byte-digit tables of the tensor-core partial rounds (poseidon_tc.cuh), t = 3 sparse schedules: per partial round k the tables of
+// c = gamma_k, alpha_k, beta_k, v_k (the lp region at off_sc0 + 1) as constants kc = 0..3.
 inline std::vector<u32> tc_tables(const Field& F, const PoseidonSchedule& S) {
     std::vector<u32> out((size_t)S.rp * kTcRoundWords, 0u);
     for (int k = 0; k < S.rp; k++)
         for (int kc = 0; kc < kTcTerms; kc++) {
             Fe c;
             memcpy(c.l, &S.consts[(size_t)(S.off_sc0 + 1 + k * (2 * S.t - 2) + kc) * 4], 32);
-            unsigned char b[32][32];                              // [i][byte n] of K8_i(c)
-            Fe z{{1ull << 32, 0, 0, 0}};                          // 2^(8i + 32) mod p
-            for (int i = 0; i < 32; i++) {
-                const Fe v = F.mul(c, z);
-                for (int n = 0; n < 32; n++) b[i][n] = (unsigned char)(v.l[n / 8] >> (8 * (n % 8)));
-                for (int d = 0; d < 8; d++) z = F.add(z, z);
-            }
-            u32* o = &out[(size_t)k * kTcRoundWords];
-            for (int nt = 0; nt < 4; nt++)
-                for (int lane = 0; lane < 32; lane++)
-                    for (int r = 0; r < 2; r++) {
-                        u32 w = 0;
-                        for (int q = 0; q < 4; q++) w |= (u32)b[tc_b_k(lane, r, q)][8 * nt + tc_b_col(lane)] << (8 * q);
-                        o[tc_tab_word(nt, kc, lane, r)] = w;
-                    }
+            tc_put_table(F, c, &out[(size_t)k * kTcRoundWords], kc, kTcTerms);
         }
+    return out;
+}
+
+// The R^-1 table of tc_redc (poseidon_tc.cuh): the plain constant 1, K8_i = 2^(8i) * 2^32 / R mod p, one constant per table.
+inline std::vector<u32> tc_rinv_table(const Field& F) {
+    std::vector<u32> out(kTcRinvWords, 0u);
+    tc_put_table(F, Fe{{1, 0, 0, 0}}, out.data(), 0, 1);
     return out;
 }
 

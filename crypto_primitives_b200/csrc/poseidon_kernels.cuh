@@ -39,14 +39,17 @@ k_poseidon_crh(PoseidonDev P, const u32* __restrict__ consts, const u32* __restr
 
 // k_poseidon_crh<F, T, SINGLE, A5> with the partial rounds' products by constants on the tensor cores (pos_permute_split with TC):
 // every warp runs while any of its lanes has a hash, so that the warp-wide IMMA sees all 32 lanes; lanes past n hash zeros and
-// store nothing.  Dynamic shared memory: the schedule, then kTcWarpWords per warp.
+// store nothing.  Dynamic shared memory: the schedule, then kTcWarpWords per warp, then the R^-1 table of the S-boxes' reductions
+// (stored after the partial rounds' tables in P.tab8).
 template <class F, int T>
 __global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
 k_poseidon_crh_tc(PoseidonDev P, const u32* __restrict__ consts, const u32* __restrict__ in, u32* __restrict__ out, long n, long len,
                   long n_out) {
     extern __shared__ __align__(16) u32 cs[];
-    __shared__ __align__(8) unsigned long long mbar;
-    tma_stage_to_smem(cs, consts, (unsigned)P.n_elems * 32u, &mbar);
+    __shared__ __align__(8) unsigned long long mbar[2];
+    u32* rinv = cs + 8 * P.n_elems + (kBlock / 32) * kTcWarpWords;
+    tma_stage_to_smem(cs, consts, (unsigned)P.n_elems * 32u, &mbar[0]);
+    tma_stage_to_smem(rinv, P.tab8 + P.rp * kTcRoundWords, kTcRinvWords * 4u, &mbar[1]);
     const u32* ct = cs + (int)threadIdx.x * P.zero;
     u32* tcbuf = cs + 8 * P.n_elems + (int)(threadIdx.x >> 5) * kTcWarpWords;
     u32 pm[8];
@@ -54,10 +57,12 @@ k_poseidon_crh_tc(PoseidonDev P, const u32* __restrict__ consts, const u32* __re
     const long stride = (long)gridDim.x * blockDim.x;
     for (long w = (long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); w < n; w += stride) {
         const long i = w + (threadIdx.x & 31u);
-        pos_hash_single<F, T, true, true>(out + 8 * n_out * i, (int)n_out, in + 8 * len * i, (int)len, P, ct, pm, tcbuf, i < n);
+        pos_hash_single<F, T, true, true>(out + 8 * n_out * i, (int)n_out, in + 8 * len * i, (int)len, P, ct, pm, tcbuf, rinv, i < n);
     }
 }
-constexpr size_t pos_tc_smem(int n_elems) { return (size_t)n_elems * 32 + (size_t)(kBlock / 32) * kTcWarpWords * 4; }
+constexpr size_t pos_tc_smem(int n_elems) {
+    return (size_t)n_elems * 32 + (size_t)(kBlock / 32) * kTcWarpWords * 4 + (size_t)kTcRinvWords * 4;
+}
 
 // CPB_POS_TC=0 (read once) runs the integer-pipe kernel k_poseidon_crh<F, T, true, true> where the tensor-core one exists, so that
 // one build can compare the two; results are the same either way.

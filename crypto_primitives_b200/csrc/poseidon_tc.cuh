@@ -9,7 +9,9 @@
 // Across a warp's 32 hashes A is 32 x 32NT (one row of operand bytes per lane) and B (32NT x 32, the table) is shared by every
 // hash: mma.m16n8k32.row.col.s32.u8.u8.s32 over 2 m-tiles, 4 n-tiles and NT k-chunks.  A partial round (t = 3) needs
 //   a' = gamma*y + alpha*a + beta*s2   (NT = 3, 24 IMMA)   and   s2' = s2 + v*y   (NT = 1, 8 IMMA).
-// Every bound is checked with exact rationals in tests/test_poseidon_tc.py.
+// The same product reduces the S-box's products (tc_redc): for T = a*b = T_lo + R*T_hi, T/R == T_hi + T_lo * R^-1 (mod p), and
+// T_lo * R^-1 is a product by the constant R^-1, through the byte-digit table of the plain constant 1 (K8_i = 2^(8i) * 2^32 / R).
+// Every bound is checked with exact rationals in tests/test_poseidon_tc.py and tests/test_poseidon_tc_redc.py.
 #pragma once
 #include "fp.cuh"
 
@@ -21,6 +23,7 @@ constexpr int kTcStageStride = 28;                       // u32 per staged row: 
                                                          // each other's banks
 constexpr int kTcCbufWords = 32 * 16;                    // C buffer: 32 rows of 16 packed column pairs
 constexpr int kTcWarpWords = 32 * kTcStageStride + kTcCbufWords;   // per-warp shared memory, 5632 B
+constexpr int kTcRinvWords = 4 * 32 * 2;                 // the R^-1 table: one constant, [n-tile][lane][b0, b1], 1 KB
 
 // Fragment maps of mma.m16n8k32 with .u8 operands (PTX ISA, "Matrix Fragments for mma.m16n8k32"), g = lane >> 2, t = lane & 3:
 //   A (16 x 32, .row): register r (0..3), byte q  ->  row g + 8 (r & 1),  k 4t + q + 16 (r >> 1)
@@ -36,8 +39,9 @@ CPB_HD int tc_c_col(int lane, int r) { return 2 * (lane & 3) + (r & 1); }
 // 4t .. 4t+3 of matrix m.  Matrix m is rows 8 (m & 1) .. +7, bytes 16 (m >> 1) .. +15 of the 16 x 32 tile, so register m is A's.
 CPB_HD int tc_ldsm_row(int lane) { return (lane & 7) + 8 * ((lane >> 3) & 1); }
 CPB_HD int tc_ldsm_half(int lane) { return lane >> 4; }
-// u32 index, in a round's table, of lane's B register r for n-tile nt and k-chunk kc (host::tc_tables writes, the kernel reads).
-CPB_HD int tc_tab_word(int nt, int kc, int lane, int r) { return ((nt * kTcTerms + kc) * 32 + lane) * 2 + r; }
+// u32 index, in a table of `terms` constants (a round's kTcTerms, or the R^-1 table's one), of lane's B register r for n-tile nt
+// and k-chunk kc (host::tc_tables and host::tc_rinv_table write, the kernel reads).
+CPB_HD int tc_tab_word(int nt, int kc, int lane, int r, int terms = kTcTerms) { return ((nt * terms + kc) * 32 + lane) * 2 + r; }
 // C buffer: row `row` keeps the packed column pairs of thread-in-group t (one word per n-tile) in 16-byte chunk
 // t ^ ((row >> 1) & 3), so that the 128-bit stores by fragment and the 128-bit loads by row are both free of bank conflicts.
 CPB_HD int tc_cbuf_chunk(int row, int t) { return t ^ ((row >> 1) & 3); }
@@ -79,10 +83,21 @@ CPB_D void tc_mma(u32 (&c)[4], const u32 (&a)[4], uint2 b) {
         : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b.x), "r"(b.y));
 }
 
-// One output of the round for lane's hash: the GEMM over k-chunks KC0 .. KC0+NT-1 of the table against the staged operands
+// Where tc_output reads its B fragments: a partial round's tables in global memory through the read-only path, or the R^-1 table
+// staged in shared memory.
+struct TcTabGlobal {
+    static constexpr int kTerms = kTcTerms;
+    static CPB_D uint2 ld(const u32* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
+};
+struct TcTabShared {
+    static constexpr int kTerms = 1;
+    static CPB_D uint2 ld(const u32* p) { return *reinterpret_cast<const uint2*>(p); }
+};
+
+// One output for lane's hash: the GEMM over k-chunks KC0 .. KC0+NT-1 of the table (read through B) against the staged operands
 // 0 .. NT-1, packed, moved to one row per lane through the C buffer, rebuilt and reduced by tc_finish.  m-tile outer, so that only
-// one m-tile's A fragments (4 NT registers) and packed results (8) are live.
-template <class F, int NT, int KC0, bool U>
+// one m-tile's A fragments (4 NT registers) and packed results (8) are live.  Every lane has read the stage when it returns.
+template <class F, class B, int NT, int KC0, bool U>
 CPB_D void tc_output(u32* r, const u32* stage, u32* cbuf, const u32* tab, int lane, const u32* y, const u32* pm) {
     const int g = lane >> 2, t = lane & 3;
 #pragma unroll
@@ -97,7 +112,7 @@ CPB_D void tc_output(u32* r, const u32* stage, u32* cbuf, const u32* tab, int la
             u32 c[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
             for (int kc = 0; kc < NT; kc++)
-                tc_mma(c, a[kc], __ldg(reinterpret_cast<const uint2*>(tab + tc_tab_word(nt, KC0 + kc, lane, 0))));
+                tc_mma(c, a[kc], B::ld(tab + tc_tab_word(nt, KC0 + kc, lane, 0, B::kTerms)));
             pk[0][nt] = c[0] + (c[1] << 8);             // columns 2t, 2t + 1: 16-bit digit 4 nt + t of the row's V
             pk[1][nt] = c[2] + (c[3] << 8);
         }
@@ -132,12 +147,24 @@ template <class F> CPB_D void tc_partial_round(u32 (&an)[8], u32 (&s)[3][8], con
         *reinterpret_cast<uint4*>(stage + lane * kTcStageStride + 8 * j + 4) = make_uint4(s[j][4], s[j][5], s[j][6], s[j][7]);
     }
     __syncwarp();
-    tc_output<F, 3, 0, false>(an, stage, cbuf, tab, lane, nullptr, pm);
+    tc_output<F, TcTabGlobal, 3, 0, false>(an, stage, cbuf, tab, lane, nullptr, pm);
     u32 w[8];
-    tc_output<F, 1, 3, true>(w, stage, cbuf, tab, lane, s[2], pm);
+    tc_output<F, TcTabGlobal, 1, 3, true>(w, stage, cbuf, tab, lane, s[2], pm);
     detail::reduce8<F, 1, 1>(w);
     fp_copy(s[2], w);
     __syncwarp();                                       // every lane has read the staged operands: the next round may restage
+}
+
+// r == T/R (mod p) for the 32 hashes of a converged warp, lane's 512-bit T (fp_sqr_wide, fp_mul_wide): T_lo * R^-1 on the tensor
+// cores over the R^-1 table rinv (shared memory, host::tc_rinv_table), with T_hi as the unit addend of its reduction row.
+//   r < T_hi + p * (1 + 32 * 255 * 2^-32) <= T/R + p * (1 + 32 * 255 * 2^-32), not reduced (the CIOS rows: below T/R + p).
+// tc_finish needs T_hi + p * (1 + 2^-19) < 2^256.  buf: the warp's kTcWarpWords; the stage is free again when this returns.
+template <class F> CPB_D void tc_redc(u32* r, const u32 (&T)[16], const u32* rinv, u32* buf, const u32* pm) {
+    const int lane = threadIdx.x & 31;
+    *reinterpret_cast<uint4*>(buf + lane * kTcStageStride) = make_uint4(T[0], T[1], T[2], T[3]);
+    *reinterpret_cast<uint4*>(buf + lane * kTcStageStride + 4) = make_uint4(T[4], T[5], T[6], T[7]);
+    __syncwarp();
+    tc_output<F, TcTabShared, 1, 0, true>(r, buf, buf + 32 * kTcStageStride, rinv, lane, T + 8, pm);
 }
 #endif
 
