@@ -733,12 +733,13 @@ cpb_status cpb_poseidon_ctx_create(int field_id, int rate, int capacity, int ful
     c->sched = host::derive_schedule(F, P, true);
     c->dev = to_dev(c->sched);
     // Byte-digit tables of the tensor-core hash kernel: only where it exists (pos_alpha5_kernel; BN254 Fr, t = 3, alpha = 5).  The
-    // partial rounds' tables, then the R^-1 table that k_poseidon_crh_tc stages into shared memory.
+    // partial rounds' tables, the R^-1 table that k_poseidon_crh_tc stages into shared memory, then the full rounds' row tables.
     std::vector<u32> tab8;
     if (field_id == Bn254_Fr::ID && t == 3 && alpha == 5 && c->sched.sparse) {
         tab8 = host::tc_tables(F, c->sched);
-        const std::vector<u32> rinv = host::tc_rinv_table(F);
+        const std::vector<u32> rinv = host::tc_rinv_table(F), full = host::tc_full_tables(F, c->sched);
         tab8.insert(tab8.end(), rinv.begin(), rinv.end());
+        tab8.insert(tab8.end(), full.begin(), full.end());
     }
     size_t bytes = c->sched.consts.size() * 8, tab_bytes = c->sched.tabs.size() * 8, tab8_bytes = tab8.size() * 4;
     if (bytes > 200 * 1024) { delete c; return fail(CPB_UNSUPPORTED, "round schedule (%zu B) exceeds shared memory", bytes); }

@@ -26,8 +26,9 @@ struct PoseidonDev {
     // constants through them (fp_dot_tab).  Every device context has them; a CPU build of this code driven without them
     // (nullptr) multiplies by the Montgomery rows of `cs` instead, as the merged loop and the team kernel always do.
     const u32* tab = nullptr;
-    // Byte-digit tables of the partial rounds (host::tc_tables, poseidon_tc.cuh) in global memory, for the tensor-core hash kernel
-    // (k_poseidon_crh_tc); uploaded only for the BN254 Fr t = 3 alpha = 5 sparse schedule, nullptr otherwise.
+    // Byte-digit tables (poseidon_tc.cuh) in global memory, for the tensor-core hash kernel (k_poseidon_crh_tc): the partial rounds'
+    // (host::tc_tables), the R^-1 table (host::tc_rinv_table), then the full rounds' rows (host::tc_full_tables).  Uploaded only for
+    // the BN254 Fr t = 3 alpha = 5 sparse schedule, nullptr otherwise.
     const u32* tab8 = nullptr;
 };
 
@@ -47,12 +48,15 @@ CPB_HD bool pos_has_tables(const PoseidonDev& P) {
     return P.tab != nullptr;
 #endif
 }
+// Which matrix full round fr multiplies by in the split form: 0 M, 1 Mpre (the last first-half round), 2 Mpost (the first
+// second-half round) -- the order of the digit tables and of the tensor-core row tables.
+CPB_HD int pos_full_index(const PoseidonDev& P, int fr) {
+    const int half = P.rf / 2;
+    return fr == half - 1 ? 1 : fr == half ? 2 : 0;
+}
 // Element offsets (x 8 limbs) of the digit tables of the full-round matrix of round fr, of the per-round partial constants and
 // of the entry row (PoseidonSchedule::tabs): M, Mpre, Mpost, then the off_sc0 + 1 region; 8 elements per constant.
-CPB_HD int pos_full_table(const PoseidonDev& P, int fr) {
-    const int half = P.rf / 2;
-    return 8 * P.t * P.t * (fr == half - 1 ? 1 : fr == half ? 2 : 0);
-}
+CPB_HD int pos_full_table(const PoseidonDev& P, int fr) { return 8 * P.t * P.t * pos_full_index(P, fr); }
 
 template <class F, int T> CPB_HD void pos_add_vec(u32 (&s)[T][8], const u32* c) {
 #pragma unroll
@@ -161,8 +165,9 @@ struct PermuteHint {
 
 // A5: the exponent is 5, known at compile time (P.alpha is not read).  Every S-box is then the straight-line pos_sbox5, with no
 // run-time exponent test and no generic square-and-multiply body in either loop.
-// TC (device only, BN254 Fr t = 3 with A5): the partial rounds' products by constants run on the tensor cores (tc_partial_round,
-// poseidon_tc.cuh) over P.tab8, with the same result ranges as the table path, and every S-box reduces its products there
+// TC (device only, BN254 Fr t = 3 with A5): the partial rounds' products by constants and the full rounds' dense rows run on the
+// tensor cores (tc_partial_round, tc_full_round; poseidon_tc.cuh) over P.tab8, with the same result ranges as the table path (the
+// rows return canonical values, as fp_dot_tab), and every S-box reduces its products there
 // (pos_sbox5_tc over the R^-1 table tcrinv in shared memory).  The whole warp must be converged and run the same schedule; tcbuf
 // is the warp's kTcWarpWords of shared memory.
 template <class F, int T, bool A5 = false, bool TC = false>
@@ -208,9 +213,17 @@ CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* c
                 else pos_sbox<F>(s[0], P.alpha, top_bit, pm, lazy);
                 pos_rotl<T>(s);
             }
+            const bool entry = phase == 0 && q == cnt - 1;                                 // Mpre: row 1 of the split form
+            if constexpr (TC) {
+#if defined(__CUDA_ARCH__)
+                const u32* tf = P.tab8 + P.rp * kTcRoundWords + kTcRinvWords;               // host::tc_full_tables
+                const u32* trow = tf + 3 * kTcRowWords * pos_full_index(P, phase * half + q);
+                tc_full_round<F>(s, trow, entry ? tf + 9 * kTcRowWords : trow + kTcRowWords, need, tcbuf, pm);
+#endif
+                continue;
+            }
             const u32* rows = cs + 8 * pos_full_matrix(P, phase * half + q);
             const u32* trows = tb + 8 * pos_full_table(P, phase * half + q);
-            const bool entry = phase == 0 && q == cnt - 1;                                 // Mpre: row 1 of the split form
             // Row collector, zeroed per round so that it is dead in the partial-round loop (24 registers at t = 3, which the
             // table rows of fp_dot_tab need there) and the shift below never reads an indeterminate value.
             u32 n[T][8];

@@ -414,6 +414,23 @@ inline std::vector<u32> tc_tables(const Field& F, const PoseidonSchedule& S) {
     return out;
 }
 
+// Byte-digit tables of the tensor-core full rounds (tc_full_round, poseidon_tc.cuh), t = 3 sparse schedules: kTcFullRows tables of
+// kTcRowWords, one per dense row the split form reads -- rows 0..2 of M, Mpre and Mpost (pos_full_index order), then the entry row
+// (the lp region's Mpre row 1) -- with constant kc = j the coefficient of lane j.
+inline std::vector<u32> tc_full_tables(const Field& F, const PoseidonSchedule& S) {
+    std::vector<u32> out((size_t)kTcFullRows * kTcRowWords, 0u);
+    const int mats[3] = {S.off_m, S.off_mpre, S.off_mpre + S.t * S.t};
+    for (int row = 0; row < kTcFullRows; row++) {
+        const int off = row < 9 ? mats[row / 3] + 3 * (row % 3) : S.off_sc0 + 1 + S.rp * (2 * S.t - 2);
+        for (int kc = 0; kc < 3; kc++) {
+            Fe c;
+            memcpy(c.l, &S.consts[(size_t)(off + kc) * 4], 32);
+            tc_put_table(F, c, &out[(size_t)row * kTcRowWords], kc, 3);
+        }
+    }
+    return out;
+}
+
 // The R^-1 table of tc_redc (poseidon_tc.cuh): the plain constant 1, K8_i = 2^(8i) * 2^32 / R mod p, one constant per table.
 inline std::vector<u32> tc_rinv_table(const Field& F) {
     std::vector<u32> out(kTcRinvWords, 0u);

@@ -11,7 +11,10 @@
 //   a' = gamma*y + alpha*a + beta*s2   (NT = 3, 24 IMMA)   and   s2' = s2 + v*y   (NT = 1, 8 IMMA).
 // The same product reduces the S-box's products (tc_redc): for T = a*b = T_lo + R*T_hi, T/R == T_hi + T_lo * R^-1 (mod p), and
 // T_lo * R^-1 is a product by the constant R^-1, through the byte-digit table of the plain constant 1 (K8_i = 2^(8i) * 2^32 / R).
-// Every bound is checked with exact rationals in tests/test_poseidon_tc.py and tests/test_poseidon_tc_redc.py.
+// A full round's dense rows (tc_full_round) are NT = 3 products of the three S-box outputs, one per row, brought to [0, p) by one
+// conditional subtraction.
+// Every bound is checked with exact rationals in tests/test_poseidon_tc.py, tests/test_poseidon_tc_redc.py and
+// tests/test_poseidon_tc_full.py.
 #pragma once
 #include "fp.cuh"
 
@@ -24,6 +27,8 @@ constexpr int kTcStageStride = 28;                       // u32 per staged row: 
 constexpr int kTcCbufWords = 32 * 16;                    // C buffer: 32 rows of 16 packed column pairs
 constexpr int kTcWarpWords = 32 * kTcStageStride + kTcCbufWords;   // per-warp shared memory, 5632 B
 constexpr int kTcRinvWords = 4 * 32 * 2;                 // the R^-1 table: one constant, [n-tile][lane][b0, b1], 1 KB
+constexpr int kTcRowWords = 4 * 3 * 32 * 2;              // a full-round row's table: 3 constants, [n-tile][k-chunk][lane][b0, b1], 3 KB
+constexpr int kTcFullRows = 10;                          // the rows of M, Mpre, Mpost (3 each), then the entry row
 
 // Fragment maps of mma.m16n8k32 with .u8 operands (PTX ISA, "Matrix Fragments for mma.m16n8k32"), g = lane >> 2, t = lane & 3:
 //   A (16 x 32, .row): register r (0..3), byte q  ->  row g + 8 (r & 1),  k 4t + q + 16 (r >> 1)
@@ -39,8 +44,8 @@ CPB_HD int tc_c_col(int lane, int r) { return 2 * (lane & 3) + (r & 1); }
 // 4t .. 4t+3 of matrix m.  Matrix m is rows 8 (m & 1) .. +7, bytes 16 (m >> 1) .. +15 of the 16 x 32 tile, so register m is A's.
 CPB_HD int tc_ldsm_row(int lane) { return (lane & 7) + 8 * ((lane >> 3) & 1); }
 CPB_HD int tc_ldsm_half(int lane) { return lane >> 4; }
-// u32 index, in a table of `terms` constants (a round's kTcTerms, or the R^-1 table's one), of lane's B register r for n-tile nt
-// and k-chunk kc (host::tc_tables and host::tc_rinv_table write, the kernel reads).
+// u32 index, in a table of `terms` constants (a partial round's kTcTerms, a full-round row's 3, or the R^-1 table's one), of lane's
+// B register r for n-tile nt and k-chunk kc (host::tc_tables, host::tc_full_tables and host::tc_rinv_table write, the kernel reads).
 CPB_HD int tc_tab_word(int nt, int kc, int lane, int r, int terms = kTcTerms) { return ((nt * terms + kc) * 32 + lane) * 2 + r; }
 // C buffer: row `row` keeps the packed column pairs of thread-in-group t (one word per n-tile) in 16-byte chunk
 // t ^ ((row >> 1) & 3), so that the 128-bit stores by fragment and the 128-bit loads by row are both free of bank conflicts.
@@ -83,10 +88,10 @@ CPB_D void tc_mma(u32 (&c)[4], const u32 (&a)[4], uint2 b) {
         : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b.x), "r"(b.y));
 }
 
-// Where tc_output reads its B fragments: a partial round's tables in global memory through the read-only path, or the R^-1 table
-// staged in shared memory.
-struct TcTabGlobal {
-    static constexpr int kTerms = kTcTerms;
+// Where tc_output reads its B fragments: tables of NT constants in global memory through the read-only path (a partial round's
+// kTcTerms, a full-round row's 3), or the R^-1 table staged in shared memory.
+template <int NT> struct TcTabGlobal {
+    static constexpr int kTerms = NT;
     static CPB_D uint2 ld(const u32* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
 };
 struct TcTabShared {
@@ -137,22 +142,47 @@ CPB_D void tc_output(u32* r, const u32* stage, u32* cbuf, const u32* tab, int la
 //   an = gamma*y + alpha*a + beta*s2, below p * (1 + 3 * 255 * 2^-27) (the LAZY fp_dot_tab contract: not reduced);
 //   s2 <- s2 + v*y for s2 in [0, 2p): below p * (3 + 255 * 2^-27) after the row, one conditional subtraction of 2p (WC).
 // tab: this round's kTcRoundWords, buf: the warp's kTcWarpWords of shared memory.
-template <class F> CPB_D void tc_partial_round(u32 (&an)[8], u32 (&s)[3][8], const u32* tab, u32* buf, const u32* pm) {
-    const int lane = threadIdx.x & 31;
-    u32* stage = buf;
-    u32* cbuf = buf + 32 * kTcStageStride;
+// Stages lane's three operands s[0..2] as its row of the A operand (bytes 32 j .. 32 j + 31: s[j]) for the warp's products.
+CPB_D void tc_stage3(u32* stage, const u32 (&s)[3][8], int lane) {
 #pragma unroll
     for (int j = 0; j < 3; j++) {
         *reinterpret_cast<uint4*>(stage + lane * kTcStageStride + 8 * j) = make_uint4(s[j][0], s[j][1], s[j][2], s[j][3]);
         *reinterpret_cast<uint4*>(stage + lane * kTcStageStride + 8 * j + 4) = make_uint4(s[j][4], s[j][5], s[j][6], s[j][7]);
     }
     __syncwarp();
-    tc_output<F, TcTabGlobal, 3, 0, false>(an, stage, cbuf, tab, lane, nullptr, pm);
+}
+
+template <class F> CPB_D void tc_partial_round(u32 (&an)[8], u32 (&s)[3][8], const u32* tab, u32* buf, const u32* pm) {
+    const int lane = threadIdx.x & 31;
+    u32* stage = buf;
+    u32* cbuf = buf + 32 * kTcStageStride;
+    tc_stage3(stage, s, lane);
+    tc_output<F, TcTabGlobal<kTcTerms>, 3, 0, false>(an, stage, cbuf, tab, lane, nullptr, pm);
     u32 w[8];
-    tc_output<F, TcTabGlobal, 1, 3, true>(w, stage, cbuf, tab, lane, s[2], pm);
+    tc_output<F, TcTabGlobal<kTcTerms>, 1, 3, true>(w, stage, cbuf, tab, lane, s[2], pm);
     detail::reduce8<F, 1, 1>(w);
     fp_copy(s[2], w);
     __syncwarp();                                       // every lane has read the staged operands: the next round may restage
+}
+
+// A full round's dense rows for the 32 hashes of a converged warp, lane's S-box outputs in s (any values below 2^256, so the lazy
+// outputs below 1.24p enter as they are): s[i] <- row_i . s, canonical, for every row i with bit i of need set, and zero for the
+// others.  rows: the round matrix's three row tables, kTcRowWords apart (host::tc_full_tables); row1: the table row 1 reads (rows +
+// kTcRowWords, or the entry row).  A row's product is below p * (1 + 3 * 255 * 2^-27) < 2p, so one conditional subtraction makes it
+// canonical.  need must be the same in every lane.  buf: the warp's kTcWarpWords; the stage is free again when this returns.
+template <class F> CPB_D void tc_full_round(u32 (&s)[3][8], const u32* rows, const u32* row1, unsigned need, u32* buf, const u32* pm) {
+    const int lane = threadIdx.x & 31;
+    tc_stage3(buf, s, lane);
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        if ((need >> i) & 1u) {
+            tc_output<F, TcTabGlobal<3>, 3, 0, false>(s[i], buf, buf + 32 * kTcStageStride, i == 1 ? row1 : rows + i * kTcRowWords,
+                                                      lane, nullptr, pm);
+            fp_final_sub<F>(s[i]);
+        } else {
+            fp_zero(s[i]);
+        }
+    }
 }
 
 // r == T/R (mod p) for the 32 hashes of a converged warp, lane's 512-bit T (fp_sqr_wide, fp_mul_wide): T_lo * R^-1 on the tensor
