@@ -734,24 +734,41 @@ cpb_status cpb_poseidon_ctx_create(int field_id, int rate, int capacity, int ful
     c->dev = to_dev(c->sched);
     // Byte-digit tables of the tensor-core hash kernel: only where it exists (pos_alpha5_kernel; BN254 Fr, t = 3, alpha = 5).  The
     // partial rounds' tables, the R^-1 table that k_poseidon_crh_tc stages into shared memory, then the full rounds' row tables.
+    // With them, the compact constant image that kernel stages (host::tc_const_image).
     std::vector<u32> tab8;
+    host::TcConstImage img;
     if (field_id == Bn254_Fr::ID && t == 3 && alpha == 5 && c->sched.sparse) {
         tab8 = host::tc_tables(F, c->sched);
         const std::vector<u32> rinv = host::tc_rinv_table(F), full = host::tc_full_tables(F, c->sched);
         tab8.insert(tab8.end(), rinv.begin(), rinv.end());
         tab8.insert(tab8.end(), full.begin(), full.end());
+        img = host::tc_const_image(c->sched);
     }
-    size_t bytes = c->sched.consts.size() * 8, tab_bytes = c->sched.tabs.size() * 8, tab8_bytes = tab8.size() * 4;
+    size_t bytes = c->sched.consts.size() * 8, tab_bytes = c->sched.tabs.size() * 8, tab8_bytes = tab8.size() * 4,
+           img_bytes = img.consts.size() * 8;
     if (bytes > 200 * 1024) { delete c; return fail(CPB_UNSUPPORTED, "round schedule (%zu B) exceeds shared memory", bytes); }
-    // staged schedule, then the digit tables and the byte-digit tables (global memory)
-    cudaError_t e = cudaMalloc(&c->d_consts, bytes + tab_bytes + tab8_bytes);
+    // staged schedule, then the digit tables, the byte-digit tables and the compact image (global memory)
+    cudaError_t e = cudaMalloc(&c->d_consts, bytes + tab_bytes + tab8_bytes + img_bytes);
     if (e == cudaSuccess) e = cudaMemcpy(c->d_consts, c->sched.consts.data(), bytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess && tab_bytes)
         e = cudaMemcpy(c->d_consts + bytes / 4, c->sched.tabs.data(), tab_bytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess && tab8_bytes)
         e = cudaMemcpy(c->d_consts + (bytes + tab_bytes) / 4, tab8.data(), tab8_bytes, cudaMemcpyHostToDevice);
     if (tab_bytes) c->dev.tab = c->d_consts + bytes / 4;
+    if (e == cudaSuccess && img_bytes)
+        e = cudaMemcpy(c->d_consts + (bytes + tab_bytes + tab8_bytes) / 4, img.consts.data(), img_bytes, cudaMemcpyHostToDevice);
     if (tab8_bytes) c->dev.tab8 = c->d_consts + (bytes + tab_bytes) / 4;
+    if (img_bytes) {
+        c->dev_tc = c->dev;
+        c->dev_tc.off_c = img.off_c;
+        c->dev_tc.off_cp0 = img.off_cp0;
+        c->dev_tc.off_pc = img.off_pc;
+        c->dev_tc.off_mod = img.off_mod;
+        c->dev_tc.off_sc0 = img.off_sc0;
+        c->dev_tc.n_elems = img.n_elems;
+        c->dev_tc.off_m = c->dev_tc.off_mpre = c->dev_tc.off_sp = c->dev_tc.off_arkp = -1;   // not in the image
+        c->d_tc_consts = c->d_consts + (bytes + tab_bytes + tab8_bytes) / 4;
+    }
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) {
         if (c->d_consts) cudaFree(c->d_consts);

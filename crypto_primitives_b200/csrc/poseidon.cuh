@@ -169,10 +169,12 @@ struct PermuteHint {
 // tensor cores (tc_partial_round, tc_full_round; poseidon_tc.cuh) over P.tab8, with the same result ranges as the table path (the
 // rows return canonical values, as fp_dot_tab), and every S-box reduces its products there
 // (pos_sbox5_tc over the R^-1 table tcrinv in shared memory).  The whole warp must be converged and run the same schedule; tcbuf
-// is the warp's kTcWarpWords of shared memory.
+// is the warp's kTcWarpWords of shared memory, and tcring the CTA's ring of the partial rounds' tables (TcRing).  cs and P are then
+// the compact constant image (host::tc_const_image): only the full rounds' constants, Cp0 (lane 1's entry constant in place), the
+// lane-0 partial-round constants, the modulus and S(c0) are read, at P's offsets into it.
 template <class F, int T, bool A5 = false, bool TC = false>
 CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* cs, const u32* pm, const PermuteHint& H,
-                              u32* tcbuf = nullptr, const u32* tcrinv = nullptr) {
+                              u32* tcbuf = nullptr, const u32* tcrinv = nullptr, TcRing* tcring = nullptr) {
     const int half = P.rf / 2;
     int top_bit = 0;
     if (!A5)
@@ -248,7 +250,7 @@ CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* c
 #pragma unroll
             for (int i = 0; i < T; i++) {                                  // Cp0, lane 1's entry in the w_hat_0 basis
                 u32 c[8];
-                ld_elem(c, i == 1 ? lp_entry + 8 * T : cs + 8 * (P.off_cp0 + i));
+                ld_elem(c, i == 1 && !TC ? lp_entry + 8 * T : cs + 8 * (P.off_cp0 + i));
                 fp_add<F>(s[i], s[i], c);
             }
             const u32* row = lp;
@@ -292,7 +294,8 @@ CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* c
                 if constexpr (TC) {
                     static_assert(T == 3 && A5 && LZ && WC, "the tensor-core partial round is built for BN254 Fr, t = 3, alpha = 5");
 #if defined(__CUDA_ARCH__)
-                    tc_partial_round<F>(an, s, P.tab8 + k * kTcRoundWords, tcbuf, pm);   // an, and s[2] <- s[2] + v * y
+                    tc_partial_round<F>(an, s, tc_ring_acquire(*tcring), tcbuf, pm);   // an, and s[2] <- s[2] + v * y
+                    tc_ring_release(*tcring, k);
 #endif
                 } else {
                     if (tabs) fp_dot_tab<F, T, 0, LZ>(an, s, trow, pm);  // row = [gamma, alpha, beta[2..T-1]]
@@ -352,10 +355,10 @@ CPB_HD void pos_permute_split(u32 (&s)[T][8], const PoseidonDev& P, const u32* c
 // A5: see pos_permute_split; dense schedules take the merged loop, which reads P.alpha.
 template <class F, int T, bool A5 = false, bool TC = false>
 CPB_HD void pos_permute(u32 (&s)[T][8], const PoseidonDev& P, const u32* cs, const u32* pm, const PermuteHint& H = PermuteHint{0, ~0u},
-                        u32* tcbuf = nullptr, const u32* tcrinv = nullptr) {
+                        u32* tcbuf = nullptr, const u32* tcrinv = nullptr, TcRing* tcring = nullptr) {
     if constexpr (CPB_POS_SPLIT_FOR(F)) {
         if (P.sparse) {
-            pos_permute_split<F, T, A5, TC>(s, P, cs, pm, H, tcbuf, tcrinv);
+            pos_permute_split<F, T, A5, TC>(s, P, cs, pm, H, tcbuf, tcrinv, tcring);
             return;
         }
     }
@@ -492,7 +495,7 @@ CPB_HD void pos_sponge(u32* out, long n_out, const u32* in, long len, const Pose
 // TC: see pos_permute_split; a lane with !live (past the end of the batch) hashes a zero input and stores nothing.
 template <class F, int T, bool A5 = false, bool TC = false>
 CPB_HD void pos_hash_single(u32* out, int n_out, const u32* in, int len, const PoseidonDev& P, const u32* cs, const u32* pm,
-                            u32* tcbuf = nullptr, const u32* tcrinv = nullptr, bool live = true) {
+                            u32* tcbuf = nullptr, const u32* tcrinv = nullptr, bool live = true, TcRing* tcring = nullptr) {
     u32 s[T][8];
     const int cap = P.cap;
 #pragma unroll
@@ -501,7 +504,7 @@ CPB_HD void pos_hash_single(u32* out, int n_out, const u32* in, int len, const P
         if (live && lane >= 0 && lane < len) ld_elem(s[i], in + 8 * lane);
         else fp_zero(s[i]);
     }
-    pos_permute<F, T, A5, TC>(s, P, cs, pm, PermuteHint{1, ((1u << n_out) - 1u) << cap}, tcbuf, tcrinv);
+    pos_permute<F, T, A5, TC>(s, P, cs, pm, PermuteHint{1, ((1u << n_out) - 1u) << cap}, tcbuf, tcrinv, tcring);
 #pragma unroll
     for (int i = 0; i < T; i++) {
         const int lane = i - cap;

@@ -11,6 +11,8 @@
 //    when a required (t-1)x(t-1) minor is singular, M[0][0] = 0, or a row's w_hat[1] is zero (the
 //    split loop carries lane 1 as w_hat . s and divides by it), the schedule falls back to the dense form.
 #pragma once
+#include <algorithm>
+
 #include "hostfp.hpp"
 #include "poseidon_tc.cuh"
 
@@ -429,6 +431,32 @@ inline std::vector<u32> tc_full_tables(const Field& F, const PoseidonSchedule& S
         }
     }
     return out;
+}
+
+// The constants k_poseidon_crh_tc stages instead of the schedule: those the tensor-core path of pos_permute_split reads, at offsets
+// of their own -- the full rounds' constants (rf x t), Cp0 with lane 1's entry constant in the w_hat_0 basis in place of lane 1's
+// (the lp region's last element, which the integer paths read at lp_entry + t), the lane-0 constants of the partial rounds, the
+// modulus and S(c0).  t = 3 sparse schedules; the other kernels keep the whole schedule.
+struct TcConstImage {
+    std::vector<u64> consts;       // 4 Montgomery limbs per element, as PoseidonSchedule::consts
+    int off_c = 0, off_cp0 = 0, off_pc = 0, off_mod = 0, off_sc0 = 0, n_elems = 0;
+};
+inline TcConstImage tc_const_image(const PoseidonSchedule& S) {
+    TcConstImage I;
+    auto push = [&](int off, int cnt) {
+        const int at = (int)(I.consts.size() / 4);
+        I.consts.insert(I.consts.end(), S.consts.begin() + (size_t)off * 4, S.consts.begin() + (size_t)(off + cnt) * 4);
+        return at;
+    };
+    I.off_c = push(S.off_c, S.rf * S.t);
+    I.off_cp0 = push(S.off_cp0, S.t);
+    const size_t entry = (size_t)(S.off_sc0 + 1 + S.rp * (2 * S.t - 2) + S.t) * 4;
+    std::copy(S.consts.begin() + entry, S.consts.begin() + entry + 4, I.consts.begin() + (size_t)(I.off_cp0 + 1) * 4);
+    I.off_pc = push(S.off_pc, S.rp);
+    I.off_mod = push(S.off_mod, 1);
+    I.off_sc0 = push(S.off_sc0, 1);
+    I.n_elems = (int)(I.consts.size() / 4);
+    return I;
 }
 
 // The R^-1 table of tc_redc (poseidon_tc.cuh): the plain constant 1, K8_i = 2^(8i) * 2^32 / R mod p, one constant per table.

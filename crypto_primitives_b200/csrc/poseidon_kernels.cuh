@@ -17,6 +17,11 @@ constexpr int kBlock = 128;
 #define CPB_POS_MINB3 5
 #endif
 constexpr int pos_min_blocks(int t) { return t <= 3 ? CPB_POS_MINB3 : t <= 5 ? 3 : 1; }
+// resident CTAs per SM for k_poseidon_crh_tc (its own shared-memory footprint fits 6; measured in DESIGN §4.2)
+#ifndef CPB_POS_TC_MINB
+#define CPB_POS_TC_MINB 5
+#endif
+static_assert(kBlock / 32 == kTcRingWarps, "every warp of a k_poseidon_crh_tc CTA releases every ring slot");
 
 // SINGLE: len <= rate, 1 <= n_out <= rate, capacity >= 1 (checked by launch_crh_ft): one permutation per hash, pos_hash_single.
 // A5 (SINGLE only): alpha == 5 compiled in (pos_permute_split); launch_crh_ft picks it where pos_alpha5_kernel says it exists.
@@ -37,31 +42,53 @@ k_poseidon_crh(PoseidonDev P, const u32* __restrict__ consts, const u32* __restr
     }
 }
 
-// k_poseidon_crh<F, T, SINGLE, A5> with the partial rounds' products by constants on the tensor cores (pos_permute_split with TC):
-// every warp runs while any of its lanes has a hash, so that the warp-wide IMMA sees all 32 lanes; lanes past n hash zeros and
-// store nothing.  Dynamic shared memory: the schedule, then kTcWarpWords per warp, then the R^-1 table of the S-boxes' reductions
-// (stored after the partial rounds' tables in P.tab8).
+// k_poseidon_crh<F, T, SINGLE, A5> with the partial rounds' products by constants on the tensor cores (pos_permute_split with TC).
+// P and consts are the compact constant image (host::tc_const_image), not the schedule.  Dynamic shared memory: the image, then
+// kTcWarpWords per warp, the R^-1 table of the S-boxes' reductions (stored after the partial rounds' tables in P.tab8), then the
+// ring of the partial rounds' tables (TcRing, kTcRingSlots x kTcRoundWords).
+// The batch loop is CTA-uniform: all four warps run every batch while any thread of the CTA has a hash, so that the warp-wide IMMA
+// sees all 32 lanes and every ring slot sees four releases per round; lanes past n (whole warps, in the last batch) hash zeros and
+// store nothing.
+// No wait can deadlock.  The only waits after the staging's __syncthreads are a warp's waits for round g's table (tc_ring_acquire),
+// and every warp runs the same rounds 0 .. g_end-1 in order.  Round g's copy is issued at the start (g < kTcRingSlots) or by the
+// last of the four releases of round g - kTcRingSlots, and each warp releases that round before it waits for round g.  Take the
+// smallest round g* any warp waits for: every warp is at g* or later, or done, so all four have released g* - kTcRingSlots, the copy
+// of g* (< g_end) was issued, and it completes.  A slot's barrier cannot run a phase ahead of a waiter (round g + kTcRingSlots's copy
+// needs the waiter's own release of g), so the parity of g / kTcRingSlots names the right phase.  Copies are issued only for rounds
+// below g_end, each of which every warp waits for, so none is in flight when the CTA exits.  Each wait is bounded (trap after ~4 s).
 template <class F, int T>
-__global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
+__global__ void __launch_bounds__(kBlock, CPB_POS_TC_MINB)
 k_poseidon_crh_tc(PoseidonDev P, const u32* __restrict__ consts, const u32* __restrict__ in, u32* __restrict__ out, long n, long len,
                   long n_out) {
     extern __shared__ __align__(16) u32 cs[];
-    __shared__ __align__(8) unsigned long long mbar[2];
+    __shared__ __align__(8) unsigned long long mbar[2], full[kTcRingSlots];
+    __shared__ unsigned released[kTcRingSlots];
     u32* rinv = cs + 8 * P.n_elems + (kBlock / 32) * kTcWarpWords;
-    tma_stage_to_smem(cs, consts, (unsigned)P.n_elems * 32u, &mbar[0]);
+    const long stride = (long)gridDim.x * blockDim.x, base = (long)blockIdx.x * blockDim.x;
+    TcRing ring{rinv + kTcRinvWords, full, released, P.tab8, P.rp, 0u, n > base ? (unsigned)((n - base + stride - 1) / stride * P.rp) : 0u};
+    if (threadIdx.x == 0) {
+        for (int q = 0; q < kTcRingSlots; q++) {
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((unsigned)__cvta_generic_to_shared(full + q)));
+            released[q] = 0;
+        }
+    }
+    tma_stage_to_smem(cs, consts, (unsigned)P.n_elems * 32u, &mbar[0]);        // its fence and __syncthreads publish the ring's state
     tma_stage_to_smem(rinv, P.tab8 + P.rp * kTcRoundWords, kTcRinvWords * 4u, &mbar[1]);
+    if (threadIdx.x == 0)
+        for (int q = 0; q < kTcRingSlots && (unsigned)q < ring.g_end; q++) tc_ring_fill(ring, q, q % P.rp);
     const u32* ct = cs + (int)threadIdx.x * P.zero;
     u32* tcbuf = cs + 8 * P.n_elems + (int)(threadIdx.x >> 5) * kTcWarpWords;
     u32 pm[8];
     ld_elem(pm, ct + 8 * P.off_mod);
-    const long stride = (long)gridDim.x * blockDim.x;
-    for (long w = (long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); w < n; w += stride) {
-        const long i = w + (threadIdx.x & 31u);
-        pos_hash_single<F, T, true, true>(out + 8 * n_out * i, (int)n_out, in + 8 * len * i, (int)len, P, ct, pm, tcbuf, rinv, i < n);
+    for (long b = base; b < n; b += stride) {
+        const long i = b + threadIdx.x;
+        pos_hash_single<F, T, true, true>(out + 8 * n_out * i, (int)n_out, in + 8 * len * i, (int)len, P, ct, pm, tcbuf, rinv, i < n,
+                                          &ring);
     }
 }
 constexpr size_t pos_tc_smem(int n_elems) {
-    return (size_t)n_elems * 32 + (size_t)(kBlock / 32) * kTcWarpWords * 4 + (size_t)kTcRinvWords * 4;
+    return (size_t)n_elems * 32 + (size_t)(kBlock / 32) * kTcWarpWords * 4 + (size_t)kTcRinvWords * 4 +
+           (size_t)kTcRingSlots * kTcRoundWords * 4;
 }
 
 // CPB_POS_TC=0 (read once) runs the integer-pipe kernel k_poseidon_crh<F, T, true, true> where the tensor-core one exists, so that
@@ -101,6 +128,10 @@ struct cpb_poseidon_ctx {
     cpb::host::PoseidonSchedule sched;
     cpb::PoseidonDev dev{};
     u32* d_consts = nullptr;
+    // k_poseidon_crh_tc's compact constant image (host::tc_const_image) and its offsets; only where dev.tab8 is set.  d_tc_consts
+    // points into the d_consts allocation.
+    cpb::PoseidonDev dev_tc{};
+    const u32* d_tc_consts = nullptr;
     cudaStream_t stream = nullptr;
     std::mutex mu;
     cpb::Scratch s_in, s_out, s_aux;
@@ -150,9 +181,9 @@ cpb_status launch_crh_ft(cpb_poseidon_ctx* c, const u32* in, size_t len, u32* ou
     const bool single = len <= (size_t)c->dev.rate && n_out >= 1 && n_out <= (size_t)c->dev.rate && c->dev.cap >= 1;
     if constexpr (pos_alpha5_kernel<F, T>()) {
         if (single && c->dev.alpha == 5 && c->dev.tab8 && pos_tc_enabled()) {
-            CPB_TRY(grid_for(k_poseidon_crh_tc<F, T>, pos_tc_smem(c->dev.n_elems), c->sms, (long)n, grid));
-            k_poseidon_crh_tc<F, T><<<grid, kBlock, pos_tc_smem(c->dev.n_elems), st>>>(c->dev, c->d_consts, in, out, (long)n, (long)len,
-                                                                                       (long)n_out);
+            CPB_TRY(grid_for(k_poseidon_crh_tc<F, T>, pos_tc_smem(c->dev_tc.n_elems), c->sms, (long)n, grid));
+            k_poseidon_crh_tc<F, T><<<grid, kBlock, pos_tc_smem(c->dev_tc.n_elems), st>>>(c->dev_tc, c->d_tc_consts, in, out, (long)n,
+                                                                                          (long)len, (long)n_out);
             CPB_CUDA(cudaGetLastError());
             return CPB_OK;
         }
@@ -365,11 +396,6 @@ __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long
 }
 __device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
     asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    return t;
 }
 
 // Leading-bit indexes of alpha and alpha - 1, the exponents of team_phase1.

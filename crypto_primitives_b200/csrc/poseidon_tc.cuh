@@ -30,6 +30,29 @@ constexpr int kTcRinvWords = 4 * 32 * 2;                 // the R^-1 table: one 
 constexpr int kTcRowWords = 4 * 3 * 32 * 2;              // a full-round row's table: 3 constants, [n-tile][k-chunk][lane][b0, b1], 3 KB
 constexpr int kTcFullRows = 10;                          // the rows of M, Mpre, Mpost (3 each), then the entry row
 
+// The per-CTA ring of the partial rounds' tables (k_poseidon_crh_tc).  The CTA's four warps run the same partial rounds in the same
+// order, batch after batch, so they share one shared-memory copy of each round's table instead of each fetching it from L2.  Round
+// g of the CTA -- counted over all of its batches, so g mod rp is the partial round -- reads slot g mod kTcRingSlots once that
+// slot's "full" mbarrier has completed phase g / kTcRingSlots (one bulk copy of kTcRoundWords, verbatim from P.tab8).  A warp
+// releases round g when its last read of the slot is done; the kTcRingWarps-th release (a per-slot count) refills the slot with
+// round g + kTcRingSlots's table, unless the CTA runs no such round.  Two slots keep the CTA's shared memory under 6 CTAs per SM.
+constexpr int kTcRingSlots = 2;
+constexpr int kTcRingWarps = 4;                          // warps per CTA (kBlock / 32) that read every slot
+CPB_HD int tc_ring_slot(unsigned g) { return (int)(g % kTcRingSlots); }
+CPB_HD unsigned tc_ring_parity(unsigned g) { return (g / kTcRingSlots) & 1u; }
+// The partial round whose table the refill after partial round k brings: the one kTcRingSlots rounds later, wrapping into the
+// next hash of the batch loop.
+CPB_HD int tc_ring_next(int k, int rp) { return (k + kTcRingSlots) % rp; }
+struct TcRing {
+    u32* slots;                    // kTcRingSlots x kTcRoundWords, shared memory
+    unsigned long long* full;      // kTcRingSlots mbarriers, arrival count 1 (the refill's expect_tx), completed by the copy
+    unsigned* released;            // kTcRingSlots counters of releases; a multiple of kTcRingWarps when every warp is done
+    const u32* src;                // the partial rounds' tables (P.tab8)
+    int rp;
+    unsigned g;                    // this warp's next round
+    unsigned g_end;                // the CTA's number of rounds: batches x rp (below 2^32 for any n the grid can stride over)
+};
+
 // Fragment maps of mma.m16n8k32 with .u8 operands (PTX ISA, "Matrix Fragments for mma.m16n8k32"), g = lane >> 2, t = lane & 3:
 //   A (16 x 32, .row): register r (0..3), byte q  ->  row g + 8 (r & 1),  k 4t + q + 16 (r >> 1)
 //   B (32 x 8, .col):  register r (0..1), byte q  ->  k 4t + q + 16 r,    column g
@@ -77,6 +100,58 @@ template <class F, bool U> CPB_HD void tc_finish(u32* r, const u32 (&h)[16], con
     r[7] = addc(O[7], 0u);
 }
 
+#if defined(__CUDACC__)
+CPB_D unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+    return t;
+}
+
+// Bulk copy of partial round k's table into `slot`, completing the slot's next phase (one thread).  The proxy fence orders the
+// warps' reads of the slot, which the release count has ordered before this thread, before the copy's writes.
+CPB_D void tc_ring_fill(const TcRing& R, int slot, int k) {
+    const unsigned mb = (unsigned)__cvta_generic_to_shared(R.full + slot);
+    const unsigned dst = (unsigned)__cvta_generic_to_shared(R.slots + slot * kTcRoundWords);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(kTcRoundWords * 4) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+                 "l"(R.src + (size_t)k * kTcRoundWords), "r"(kTcRoundWords * 4), "r"(mb)
+                 : "memory");
+}
+
+// This warp's round R.g: waits (every lane) until its table has landed and returns the slot.  Bounded: trap after ~4 s.
+CPB_D const u32* tc_ring_acquire(const TcRing& R) {
+    const int slot = tc_ring_slot(R.g);
+    const unsigned mb = (unsigned)__cvta_generic_to_shared(R.full + slot), par = tc_ring_parity(R.g);
+    unsigned done = 0;
+    unsigned long long t0 = 0;
+    for (;;) {
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(done) : "r"(mb), "r"(par) : "memory");
+        if (done) break;
+        if (t0 == 0) t0 = globaltimer_ns();
+        else if (globaltimer_ns() - t0 > 4000000000ull) __trap();
+    }
+    return R.slots + slot * kTcRoundWords;
+}
+
+// This warp is done with round R.g (partial round k of its hash): lane 0 counts the release, and the last of the CTA's warps
+// refills the slot with round R.g + kTcRingSlots's table.  The block fences make the count a release / acquire pair, so every
+// warp's reads of the slot come before the refill.
+CPB_D void tc_ring_release(TcRing& R, int k) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) {
+        const int slot = tc_ring_slot(R.g);
+        __threadfence_block();
+        if (atomicAdd(R.released + slot, 1u) % kTcRingWarps == kTcRingWarps - 1 && R.g + kTcRingSlots < R.g_end) {
+            __threadfence_block();
+            tc_ring_fill(R, slot, tc_ring_next(k, R.rp));
+        }
+    }
+    R.g++;
+}
+#endif
+
 #if defined(__CUDA_ARCH__)
 CPB_D void tc_ldsm_x4(u32 (&d)[4], const u32* smem) {
     const unsigned a = (unsigned)__cvta_generic_to_shared(smem);
@@ -88,14 +163,14 @@ CPB_D void tc_mma(u32 (&c)[4], const u32 (&a)[4], uint2 b) {
         : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b.x), "r"(b.y));
 }
 
-// Where tc_output reads its B fragments: tables of NT constants in global memory through the read-only path (a partial round's
-// kTcTerms, a full-round row's 3), or the R^-1 table staged in shared memory.
+// Where tc_output reads its B fragments: tables of NT constants in global memory through the read-only path (a full-round row's 3),
+// or in shared memory (a partial round's kTcTerms in a slot of the ring, the R^-1 table's one).
 template <int NT> struct TcTabGlobal {
     static constexpr int kTerms = NT;
     static CPB_D uint2 ld(const u32* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
 };
-struct TcTabShared {
-    static constexpr int kTerms = 1;
+template <int NT> struct TcTabShared {
+    static constexpr int kTerms = NT;
     static CPB_D uint2 ld(const u32* p) { return *reinterpret_cast<const uint2*>(p); }
 };
 
@@ -141,7 +216,7 @@ CPB_D void tc_output(u32* r, const u32* stage, u32* cbuf, const u32* tab, int la
 // The partial round's products by constants for the 32 hashes of a converged warp, lane's hash in s = (y, a, s2):
 //   an = gamma*y + alpha*a + beta*s2, below p * (1 + 3 * 255 * 2^-27) (the LAZY fp_dot_tab contract: not reduced);
 //   s2 <- s2 + v*y for s2 in [0, 2p): below p * (3 + 255 * 2^-27) after the row, one conditional subtraction of 2p (WC).
-// tab: this round's kTcRoundWords, buf: the warp's kTcWarpWords of shared memory.
+// tab: this round's kTcRoundWords in shared memory (a slot of the ring), buf: the warp's kTcWarpWords of shared memory.
 // Stages lane's three operands s[0..2] as its row of the A operand (bytes 32 j .. 32 j + 31: s[j]) for the warp's products.
 CPB_D void tc_stage3(u32* stage, const u32 (&s)[3][8], int lane) {
 #pragma unroll
@@ -157,9 +232,9 @@ template <class F> CPB_D void tc_partial_round(u32 (&an)[8], u32 (&s)[3][8], con
     u32* stage = buf;
     u32* cbuf = buf + 32 * kTcStageStride;
     tc_stage3(stage, s, lane);
-    tc_output<F, TcTabGlobal<kTcTerms>, 3, 0, false>(an, stage, cbuf, tab, lane, nullptr, pm);
+    tc_output<F, TcTabShared<kTcTerms>, 3, 0, false>(an, stage, cbuf, tab, lane, nullptr, pm);
     u32 w[8];
-    tc_output<F, TcTabGlobal<kTcTerms>, 1, 3, true>(w, stage, cbuf, tab, lane, s[2], pm);
+    tc_output<F, TcTabShared<kTcTerms>, 1, 3, true>(w, stage, cbuf, tab, lane, s[2], pm);
     detail::reduce8<F, 1, 1>(w);
     fp_copy(s[2], w);
     __syncwarp();                                       // every lane has read the staged operands: the next round may restage
@@ -194,7 +269,7 @@ template <class F> CPB_D void tc_redc(u32* r, const u32 (&T)[16], const u32* rin
     *reinterpret_cast<uint4*>(buf + lane * kTcStageStride) = make_uint4(T[0], T[1], T[2], T[3]);
     *reinterpret_cast<uint4*>(buf + lane * kTcStageStride + 4) = make_uint4(T[4], T[5], T[6], T[7]);
     __syncwarp();
-    tc_output<F, TcTabShared, 1, 0, true>(r, buf, buf + 32 * kTcStageStride, rinv, lane, T + 8, pm);
+    tc_output<F, TcTabShared<1>, 1, 0, true>(r, buf, buf + 32 * kTcStageStride, rinv, lane, T + 8, pm);
 }
 #endif
 
