@@ -90,6 +90,10 @@ SIGNATURES = {
     "cpb_merkle_pedersen_update": (C.c_int, [vp, vp, u64p, u64p, C.c_size_t, u64p, u8p, C.c_size_t, C.c_size_t, u64p, C.POINTER(C.c_int)]),
     "cpb_merkle_mixed_build": (C.c_int, [vp, vp, u8p, C.c_size_t, C.c_size_t, u64p, u64p]),
     "cpb_merkle_mixed_build_dev": (C.c_int, [vp, vp, vp, C.c_size_t, C.c_size_t, C.c_size_t, vp, vp, vp]),
+    "cpb_merkle_pedersen_verify_batch": (C.c_int, [vp, vp, u64p, u8p, C.c_size_t, u64p, u64p, C.c_size_t, u64p, u8p, C.c_size_t]),
+    "cpb_merkle_pedersen_verify_batch_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, C.c_size_t, vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp]),
+    "cpb_merkle_mixed_verify_batch": (C.c_int, [vp, vp, u64p, u8p, C.c_size_t, u64p, u64p, C.c_size_t, u64p, u8p, C.c_size_t]),
+    "cpb_merkle_mixed_verify_batch_dev": (C.c_int, [vp, vp, vp, vp, C.c_size_t, C.c_size_t, vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp]),
     "cpb_exchange_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
     "cpb_exchange_destroy": (None, [vp]),
     "cpb_exchange_world": (C.c_int, [vp]),

@@ -516,15 +516,16 @@ template <class F, int T> CPB_HD void pos_crh(u32* out, const u32* in, long len,
     pos_sponge<F, T>(out, 1, in, len, P, cs, pm);
 }
 
-// Path::verify (R/merkle_tree/mod.rs:172-212) for the field-leaf Config: hash the leaf, fold the
-// authentication path bottom-up choosing sides by the index bits, compare with the root.
-// auth_path: plen elements ordered root side first (as Path.auth_path).  PL/PN, cl/cn: leaf / node schedules.
+// The fold of Path::verify (R/merkle_tree/mod.rs:172-212) from a claimed leaf digest: the digest and the leaf sibling, then the
+// authentication path bottom-up, each pair through poseidon::TwoToOneCRH with sides chosen by the index bits (bits above plen are
+// never read), then the comparison with the root.  auth_path: plen elements ordered root side first (as Path.auth_path).
+// PN, cn: node schedule.  Any Config whose inner hash is Poseidon and whose leaf digest is one field element folds through it.
 template <class F, int T>
-CPB_HD bool pos_verify_path(const u32* leaf, long leaf_len, const u32* sibling, const u32* auth_path, int plen, unsigned long long index,
-                            const u32* root, const PoseidonDev& PL, const u32* cl, const PoseidonDev& PN, const u32* cn, const u32* pm) {
+CPB_HD bool pos_verify_digest(const u32* digest, const u32* sibling, const u32* auth_path, int plen, unsigned long long index,
+                              const u32* root, const PoseidonDev& PN, const u32* cn, const u32* pm) {
     alignas(16) u32 pair[16];        // read back through 128-bit loads
     u32 cur[8];
-    pos_crh<F, T>(cur, leaf, leaf_len, PL, cl, pm);
+    ld_elem(cur, digest);
     u32 sib[8];
     ld_elem(sib, sibling);
 #pragma unroll 1
@@ -542,6 +543,15 @@ CPB_HD bool pos_verify_path(const u32* leaf, long leaf_len, const u32* sibling, 
     u32 r[8];
     ld_elem(r, root);
     return fp_eq(cur, r);
+}
+
+// Path::verify for the field-leaf Config: hash the leaf (PL, cl: leaf schedule), then pos_verify_digest.
+template <class F, int T>
+CPB_HD bool pos_verify_path(const u32* leaf, long leaf_len, const u32* sibling, const u32* auth_path, int plen, unsigned long long index,
+                            const u32* root, const PoseidonDev& PL, const u32* cl, const PoseidonDev& PN, const u32* cn, const u32* pm) {
+    alignas(16) u32 cur[8];          // read back through 128-bit loads
+    pos_crh<F, T>(cur, leaf, leaf_len, PL, cl, pm);
+    return pos_verify_digest<F, T>(cur, sibling, auth_path, plen, index, root, PN, cn, pm);
 }
 
 // ---- ragged batches: input i is values[offsets[i] .. offsets[i+1]), n + 1 offsets, offsets[0] not necessarily 0.

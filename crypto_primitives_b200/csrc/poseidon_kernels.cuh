@@ -250,6 +250,38 @@ cpb_status launch_verify_ft(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, cons
     return CPB_OK;
 }
 
+// One Path::verify fold per thread from an already hashed leaf (pos_verify_digest): digests[i] is proof i's claimed leaf digest.
+// Only the node schedule is staged in shared memory.  The Pedersen-leaf tree's verification (cpb_merkle_verify_pedersen.cu) runs it
+// after the Pedersen leaf hash.
+template <class F, int T>
+__global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
+k_poseidon_verify_digests(PoseidonDev PN, const u32* __restrict__ consts_n, const u32* __restrict__ root, const u32* __restrict__ digests,
+                          const u32* __restrict__ siblings, const u32* __restrict__ paths, int plen,
+                          const unsigned long long* __restrict__ indexes, unsigned char* __restrict__ ok, long n) {
+    extern __shared__ __align__(16) u32 cs[];
+    __shared__ __align__(8) unsigned long long mbar;
+    tma_stage_to_smem(cs, consts_n, (unsigned)PN.n_elems * 32u, &mbar);
+    const int z = (int)threadIdx.x * PN.zero;
+    u32 pm[8];
+    ld_elem(pm, cs + z + 8 * PN.off_mod);
+    const long stride = (long)gridDim.x * blockDim.x;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        ok[i] = pos_verify_digest<F, T>(digests + 8 * i, siblings + 8 * i, paths + 8 * (long)plen * i, plen, indexes[i], root, PN, cs + z,
+                                        pm) ? 1 : 0;
+}
+
+template <class F, int T>
+cpb_status launch_verify_digests_ft(cpb_poseidon_ctx* node, const u32* root, const u32* digests, const u32* siblings, const u32* paths,
+                                    int plen, const unsigned long long* indexes, unsigned char* ok, size_t n, cudaStream_t st) {
+    size_t smem = (size_t)node->dev.n_elems * 32;
+    int grid = 1;
+    CPB_TRY(grid_for(k_poseidon_verify_digests<F, T>, smem, node->sms, (long)n, grid));
+    k_poseidon_verify_digests<F, T><<<grid, kBlock, smem, st>>>(node->dev, node->d_consts, root, digests, siblings, paths, plen, indexes, ok,
+                                                                (long)n);
+    CPB_CUDA(cudaGetLastError());
+    return CPB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Ragged batches (poseidon.cuh: ragged_span): item i hashes values[offsets[i] - vbase ..] at its own length and writes out[i].
 // Slot j of [range[0], range[1]) is item order[j]; order == nullptr walks the items in input order and range == nullptr is
@@ -583,6 +615,14 @@ cpb_status merkle_build_streams(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, 
     template cpb_status launch_verify_ragged_ft<F, T>(cpb_poseidon_ctx*, cpb_poseidon_ctx*, const u32*, const u32*, u64, const u64*, \
                                                       const u32*, const u32*, int, const unsigned long long*, unsigned char*, size_t, \
                                                       cudaStream_t);
+// the digest fold (Pedersen-leaf / Poseidon-node trees) exists only for the fields that are a curve's base field, each in a
+// translation unit of its own (poseidon_digests_<field>.cu) for the same reason
+#define CPB_POS_INSTANTIATE_DIGESTS(F, T)                                                                                \
+    template cpb_status launch_verify_digests_ft<F, T>(cpb_poseidon_ctx*, const u32*, const u32*, const u32*, const u32*, int,   \
+                                                       const unsigned long long*, unsigned char*, size_t, cudaStream_t);
+#define CPB_POS_EXTERN_DIGESTS(F, T)                                                                                     \
+    extern template cpb_status launch_verify_digests_ft<F, T>(cpb_poseidon_ctx*, const u32*, const u32*, const u32*, const u32*, \
+                                                              int, const unsigned long long*, unsigned char*, size_t, cudaStream_t);
 #define CPB_POS_INSTANTIATE_TEAM(F) template cpb_status launch_tree_top_f<F>(cpb_poseidon_ctx*, TopJob, cudaStream_t);
 #define CPB_POS_EXTERN_TEAM(F) extern template cpb_status launch_tree_top_f<F>(cpb_poseidon_ctx*, TopJob, cudaStream_t);
 #define CPB_POS_EXTERN(F, T)                                                                                             \

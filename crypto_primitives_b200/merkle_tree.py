@@ -9,7 +9,8 @@ mod.rs:547-623.  Verification and update are LEVEL-SYNCHRONOUS device batches fo
 (or all touched nodes) of one tree level go through ONE two-to-one batch call, so k proofs / k updated
 leaves cost height launches, not k * height (`verify_paths_batch`, `MultiPath.verify`, `update_batch`);
 the Poseidon field-leaf Config additionally has a single-launch kernel that recomputes one root per
-thread (`cpb_merkle_poseidon_verify_batch`), and Configs whose inner hash is Poseidon update in ONE library
+thread (`cpb_merkle_poseidon_verify_batch`), the Pedersen byte and Pedersen-leaf / Poseidon-node trees verify in one library call
+(`cpb_merkle_pedersen_verify_batch`, `cpb_merkle_mixed_verify_batch`: no host round trip between levels), and Configs whose inner hash is Poseidon update in ONE library
 call (`cpb_merkle_poseidon_update_digests`, and `cpb_merkle_pedersen_update` for the Pedersen byte tree: every level on the
 device, only touched nodes cross PCIe).
 """
@@ -242,6 +243,31 @@ def _select_and_hash(cfg: Config, two_to_one_params, cur, sib, on_right, device)
     return cfg.two_to_one_batch(two_to_one_params, np.ascontiguousarray(pairs), device)
 
 
+def _verify_byte_leaves(cfg: Config, leaf_hash_params, two_to_one_params, root_hash, leaves, sib, paths, idx, plen, device) -> np.ndarray:
+    """n x Path::verify in ONE library call for the trees with a Pedersen leaf hash over byte leaves: the byte tree
+    (cpb_merkle_pedersen_verify_batch) and the Pedersen-leaf / Poseidon-node tree (cpb_merkle_mixed_verify_batch).  leaves: (n, leaf_len)
+    bytes; sib, paths, idx as generate_proofs_batch returns them.  A leaf longer than the window raises ValueError, as the build."""
+    w = cfg.digest_words
+    fn = N.lib.cpb_merkle_pedersen_verify_batch if type(cfg) is PedersenByteConfig else N.lib.cpb_merkle_mixed_verify_batch
+    lv = np.ascontiguousarray(leaves, dtype=np.uint8)
+    assert lv.ndim == 2, "leaves must be (n, leaf_len) bytes"
+    n = lv.shape[0]
+    ix = np.ascontiguousarray(idx, dtype=np.uint64).reshape(-1)
+    assert ix.size == n, "one leaf per proof"
+    sb = np.ascontiguousarray(sib, dtype=np.uint64).reshape(n, w)
+    ap = np.ascontiguousarray(paths, dtype=np.uint64).reshape(n, plen, w)
+    root = np.ascontiguousarray(root_hash, dtype=np.uint64).reshape(w)
+    ok = np.zeros(n, dtype=np.uint8)
+    try:
+        N.check(fn(leaf_hash_params.context(device), two_to_one_params.context(device), _p(root), lv.ctypes.data_as(N.u8p), lv.shape[1],
+                   _p(sb), _p(ap), plen, _p(ix), ok.ctypes.data_as(N.u8p), n))
+    except N.CpbError as e:
+        if e.status == N.CPB_BAD_LENGTH:
+            raise ValueError("incorrect input length") from e
+        raise
+    return ok.astype(bool)
+
+
 def verify_paths_batch(leaf_hash_params, two_to_one_params, root_hash, leaves, proofs, config: Config = None, device: int = 0) -> np.ndarray:
     """n x Path::verify (mod.rs:172-212) for any Config as device batches: one leaf-hash batch, then one two-to-one batch
     per tree level for ALL n paths (height launches in total).  `proofs`: Paths of one tree; returns a bool array."""
@@ -271,8 +297,14 @@ class Path:
 
     def verify(self, leaf_hash_params, two_to_one_params, root_hash, leaf, config: Config = None, device: int = 0) -> bool:
         """Path::verify, mod.rs:172-212.  Field-leaf Poseidon Config: ONE kernel launch recomputes the root
-        (cpb_merkle_poseidon_verify_batch with n = 1); other Configs: the level-synchronous batch with n = 1."""
+        (cpb_merkle_poseidon_verify_batch with n = 1); Pedersen byte and Pedersen-leaf / Poseidon-node trees: one library call with
+        n = 1 (cpb_merkle_pedersen_verify_batch, cpb_merkle_mixed_verify_batch); other Configs: the level-synchronous batch with n = 1."""
         cfg = config or PoseidonFieldConfig()
+        if type(cfg) in (PedersenByteConfig, PedersenPoseidonConfig):
+            plen = len(self.auth_path)
+            paths = np.stack(self.auth_path) if plen else np.zeros(0, dtype=np.uint64)
+            return bool(_verify_byte_leaves(cfg, leaf_hash_params, two_to_one_params, root_hash, np.asarray(leaf, dtype=np.uint8).reshape(1, -1),
+                                            self.leaf_sibling_hash, paths, [self.leaf_index], plen, device)[0])
         if type(cfg) is PoseidonFieldConfig:
             lv = np.ascontiguousarray(np.asarray(leaf, dtype=np.uint64).reshape(1, -1, 4))
             plen = len(self.auth_path)
@@ -429,11 +461,24 @@ class MerkleTree:
         return sib, paths, idx.astype(np.uint64)
 
     def verify_proofs_batch(self, proofs, leaves, root_hash=None) -> np.ndarray:
-        """Many Path::verify (mod.rs:172-212) in one kernel launch (field-leaf Config): proofs = list of Path for
-        `leaves[i]`, or the (siblings, paths, indexes) arrays of generate_proofs_batch; returns a bool array.
-        One GPU thread recomputes one root."""
+        """Many Path::verify (mod.rs:172-212) in one library call: proofs = list of Path for `leaves[i]`, or the (siblings, paths,
+        indexes) arrays of generate_proofs_batch; returns a bool array.  Field-leaf Config: one kernel launch, one GPU thread recomputes
+        one root.  Pedersen byte tree and Pedersen-leaf / Poseidon-node tree: leaves are (n, leaf_len) bytes; the leaf hash, then one
+        device grid per level (byte tree) or one fold kernel (Poseidon nodes), no host round trip in between."""
+        plen = self._height - 2
+        if type(self.config) in (PedersenByteConfig, PedersenPoseidonConfig):
+            if isinstance(proofs, tuple):
+                sib, paths, idx = proofs
+            else:
+                sib = np.stack([p.leaf_sibling_hash for p in proofs]) if proofs else np.zeros(0, dtype=np.uint64)
+                paths = np.stack([np.stack(p.auth_path) if plen else np.zeros(0, dtype=np.uint64) for p in proofs]) if proofs \
+                    else np.zeros(0, dtype=np.uint64)
+                idx = [p.leaf_index for p in proofs]
+            return _verify_byte_leaves(self.config, self.leaf_hash_param, self.two_to_one_hash_param, self.root() if root_hash is None else root_hash,
+                                       leaves, sib, paths, idx, plen, self.device)
         if not isinstance(self.config, PoseidonFieldConfig):
-            raise NotImplementedError("the one-launch kernel is for the Poseidon field-leaf Config; use verify_paths_batch")
+            raise NotImplementedError("one-call verification is for the Poseidon field-leaf, Pedersen byte and Pedersen-leaf / Poseidon-node "
+                                      "Configs; use verify_paths_batch")
         if R.is_ragged(leaves):                # leaves of different lengths: (values, offsets)
             lv, n_leaves = R.pack(leaves), len(leaves)
         else:

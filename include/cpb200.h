@@ -367,6 +367,52 @@ cpb_status cpb_merkle_mixed_build_dev(cpb_pedersen_ctx* leaf_ctx, cpb_poseidon_c
                                       size_t leaf_len, size_t leaf_stride, size_t n, uint64_t* leaf_nodes,
                                       uint64_t* non_leaf_nodes, void* stream);
 
+/* ---- Merkle path verification (Pedersen leaves) ------------------------------------------------------------------- */
+/* n x Path::verify (R/merkle_tree/mod.rs:172-212) for the byte tree of cpb_merkle_pedersen_build against one root (8 words,
+ * affine x, y).  Proof i = (leaf_sibling_hashes_xy[i], auth_paths_xy[i*path_len .. (i+1)*path_len) root side first as
+ * Path.auth_path, leaf_indexes[i]); ok[i] = 1 when the recomputed root equals root_xy in both coordinates, else 0.  Tree height =
+ * path_len + 2.
+ * Order of hashing, as the reference: the claimed leaf hash (pedersen::CRH of leaf i with leaf_ctx) and the leaf sibling go through
+ * TwoToOneHash::evaluate of the converted digests, sides chosen by index bit 0 (bit set: the computed node is the right child);
+ * auth-path level j = 1 .. path_len (auth_paths[i*path_len + path_len - j]) then goes through compress with bit j.  Both steps hash
+ * the 128-byte ByteDigestConverter row x_l || y_l || x_r || y_r cut to the node context's TwoToOneCRH length, as the build does.
+ * Bits of leaf_indexes[i] above path_len are ignored, as in the reference; no form rejects a large index (the verifier does not
+ * know the tree).
+ * Argument checks, on the host before any device work, in this order:
+ *   1. path_len > 62 -> CPB_BAD_PARAMS; _dev form: leaf_stride < leaf_len with n > 1 -> CPB_BAD_PARAMS;
+ *   2. a null buffer with n > 0 (leaves only when leaf_len > 0, auth_paths only when path_len > 0) -> CPB_NULL_POINTER;
+ *   3. a null context -> CPB_NULL_POINTER; leaf and node contexts on different devices or curves -> CPB_BAD_PARAMS;
+ *   4. leaf_len * 8 > WINDOW_SIZE * NUM_WINDOWS of leaf_ctx -> CPB_BAD_LENGTH, as the CRH; the node row length is checked against
+ *      node_ctx as cpb_pedersen_two_to_one_batch does.
+ * Then n == 0 returns CPB_OK without reading any array or writing `ok`.
+ * Elements are reduced Montgomery limbs; an unreduced one may give any verdict but nothing outside the caller's arrays is read or
+ * written.
+ * _dev form: every pointer is device memory, leaf i at leaves + i * leaf_stride.  No host synchronisation; scratch (192 bytes per
+ * proof) comes from the stream-ordered pool; 3 * path_len + 6 kernel launches whatever n (the leaf hash and its normalisation, per
+ * level a row kernel and the node context's hash and normalisation, a comparison), so the call can be captured in a CUDA graph.
+ * Host form: leaves packed n x leaf_len; the arrays go up on leaf_ctx's stream, the _dev code runs there, ok comes back. */
+cpb_status cpb_merkle_pedersen_verify_batch(cpb_pedersen_ctx* leaf_ctx, cpb_pedersen_ctx* node_ctx, const uint64_t* root_xy,
+                                            const uint8_t* leaves, size_t leaf_len, const uint64_t* leaf_sibling_hashes_xy,
+                                            const uint64_t* auth_paths_xy, size_t path_len, const uint64_t* leaf_indexes,
+                                            uint8_t* ok, size_t n);
+cpb_status cpb_merkle_pedersen_verify_batch_dev(cpb_pedersen_ctx* leaf_ctx, cpb_pedersen_ctx* node_ctx, const uint64_t* root_xy,
+                                                const uint8_t* leaves, size_t leaf_len, size_t leaf_stride,
+                                                const uint64_t* leaf_sibling_hashes_xy, const uint64_t* auth_paths_xy, size_t path_len,
+                                                const uint64_t* leaf_indexes, uint8_t* ok, size_t n, void* stream);
+/* The same for the tree of cpb_merkle_mixed_build: leaf digest = PedersenCRHCompressor x-coordinate (one base-field element),
+ * nodes poseidon::TwoToOneCRH; root, siblings and auth-path nodes are field elements (4 words).  Rules as above, except for the
+ * contexts: a Poseidon field that is not the curve's base field, or another device, -> CPB_BAD_PARAMS, as the mixed build; a
+ * Poseidon node rate < 2 -> CPB_UNSUPPORTED, as cpb_merkle_poseidon_verify_batch.  The _dev form takes 3 kernel launches for
+ * any path_len and n (leaf hash, normalisation, one fold kernel with one thread per proof) and 32 bytes of pool scratch per proof. */
+cpb_status cpb_merkle_mixed_verify_batch(cpb_pedersen_ctx* leaf_ctx, cpb_poseidon_ctx* node_ctx, const uint64_t* root,
+                                         const uint8_t* leaves, size_t leaf_len, const uint64_t* leaf_sibling_hashes,
+                                         const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes,
+                                         uint8_t* ok, size_t n);
+cpb_status cpb_merkle_mixed_verify_batch_dev(cpb_pedersen_ctx* leaf_ctx, cpb_poseidon_ctx* node_ctx, const uint64_t* root,
+                                             const uint8_t* leaves, size_t leaf_len, size_t leaf_stride,
+                                             const uint64_t* leaf_sibling_hashes, const uint64_t* auth_paths, size_t path_len,
+                                             const uint64_t* leaf_indexes, uint8_t* ok, size_t n, void* stream);
+
 /* ---- Merkle tree across several GPUs ------------------------------------------------------------ */
 /* The reference builds a tree in one process (MerkleTree::new, R/merkle_tree/mod.rs:411-523).  On G = 2^g GPUs the leaves
  * are sharded contiguously: rank k owns leaves [k*n/G, (k+1)*n/G), builds that subtree (its nodes in LOCAL heap order, as

@@ -228,6 +228,32 @@ public:
         return check_update_batch(leaf, two_to_one, {(uint64_t)index}, new_leaf, new_leaf.size(), asserted_new_root);
     }
 
+    // n x Path::verify (mod.rs:172-212) against `root` in one call: proofs for leaves `indexes` of this tree (generate_proof for
+    // each), `leaves` = the claimed leaves, leaf_len bytes each, back to back.  ok[i] = 1 when path i recomputes the root.
+    std::vector<uint8_t> verify_batch(const pedersen::Parameters& leaf, const pedersen::Parameters& two_to_one, const Affine& root,
+                                      const std::vector<size_t>& indexes, const std::vector<uint8_t>& leaves, size_t leaf_len) const {
+        const size_t n = indexes.size(), plen = height() - 2;
+        if (leaves.size() != n * leaf_len) throw Error(CPB_BAD_LENGTH, "one leaf of leaf_len bytes per index");
+        std::vector<Affine> sib, paths;
+        std::vector<uint64_t> idx;
+        for (size_t i : indexes) {
+            sib.push_back(leaf_nodes.at(i ^ 1));
+            std::vector<Affine> path;
+            size_t cur = (i + leaf_nodes.size() - 2) >> 1;   // parent of the leaf's position in the full tree
+            while (cur != 0) {
+                path.push_back(non_leaf_nodes[(cur & 1) ? cur + 1 : cur - 1]);
+                cur = (cur - 1) >> 1;
+            }
+            paths.insert(paths.end(), path.rbegin(), path.rend());   // root side first (compute_auth_path, mod.rs:548-573)
+            idx.push_back(i);
+        }
+        std::vector<uint8_t> ok(n, 0);
+        if (n)
+            check(cpb_merkle_pedersen_verify_batch(leaf.ctx(), two_to_one.ctx(), root.x.data(), leaves.empty() ? nullptr : leaves.data(), leaf_len,
+                                                   sib[0].x.data(), plen ? paths[0].x.data() : nullptr, plen, idx.data(), ok.data(), n));
+        return ok;
+    }
+
 private:
     bool update_impl(const pedersen::Parameters& leaf, const pedersen::Parameters& two_to_one, const std::vector<uint64_t>& indexes,
                      const std::vector<uint8_t>& leaves, size_t leaf_len, const Affine* asserted) {

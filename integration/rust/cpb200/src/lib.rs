@@ -345,6 +345,10 @@ pub mod pedersen {
         fn cpb_merkle_pedersen_update(leaf: *mut cpb_pedersen_ctx, node: *mut cpb_pedersen_ctx, leaf_nodes_xy: *mut u64,
                                       non_leaf_nodes_xy: *mut u64, n: usize, indexes: *const u64, new_leaves: *const u8, leaf_len: usize,
                                       k: usize, asserted_root_xy: *const u64, applied: *mut c_int) -> c_int;
+        // n x Path::verify of a byte tree against one root; ok[i] = 1 when path i recomputes it
+        fn cpb_merkle_pedersen_verify_batch(leaf: *mut cpb_pedersen_ctx, node: *mut cpb_pedersen_ctx, root_xy: *const u64, leaves: *const u8,
+                                            leaf_len: usize, leaf_sibling_hashes_xy: *const u64, auth_paths_xy: *const u64, path_len: usize,
+                                            leaf_indexes: *const u64, ok: *mut u8, n: usize) -> c_int;
     }
 
     struct Ctx(*mut cpb_pedersen_ctx);
@@ -461,6 +465,36 @@ pub mod pedersen {
         pub fn check_update(&mut self, leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, index: usize, new_leaf: &[u8],
                             asserted_new_root: &EdwardsAffine) -> Result<bool, Error> {
             self.check_update_batch(leaf, two_to_one, &[index], &[new_leaf.to_vec()], asserted_new_root)
+        }
+        /// n x `Path::verify` (R/merkle_tree/mod.rs:172-212) against `root` in one call: the proofs of leaves `indexes` of this tree
+        /// (`generate_proof` for each) with the claimed `leaves`, of one byte length; element i says whether path i recomputes the root.
+        /// The claimed leaves and every level are hashed on the GPU, with no host round trip between levels.
+        pub fn verify_batch(&self, leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, root: &EdwardsAffine, indexes: &[usize],
+                            leaves: &[Vec<u8>]) -> Result<Vec<bool>, Error> {
+            assert_eq!(indexes.len(), leaves.len(), "one claimed leaf per index");
+            let leaf_len = leaves.first().map_or(0, |l| l.len());
+            assert!(leaves.iter().all(|l| l.len() == leaf_len), "claimed leaves of one length");
+            let (n_leaves, plen) = (self.leaf_nodes.len(), self.height - 2);
+            let (mut sib, mut paths) = (Vec::with_capacity(indexes.len()), Vec::with_capacity(indexes.len() * plen));
+            for &i in indexes {
+                sib.push(self.leaf_nodes[i ^ 1]);
+                let mut path = Vec::with_capacity(plen);
+                let mut cur = (i + n_leaves - 2) >> 1;          // parent of the leaf's position in the full tree
+                while cur != 0 {
+                    path.push(self.non_leaf_nodes[if cur & 1 == 1 { cur + 1 } else { cur - 1 }]);
+                    cur = (cur - 1) >> 1;
+                }
+                paths.extend(path.into_iter().rev());           // root side first, as Path.auth_path
+            }
+            let idx: Vec<u64> = indexes.iter().map(|&i| i as u64).collect();
+            let flat: Vec<u8> = leaves.concat();
+            let (sib, paths, root) = (affine_limbs(&sib), affine_limbs(&paths), affine_limbs(&[*root]));
+            let mut ok = vec![0u8; idx.len()];
+            check(unsafe {
+                cpb_merkle_pedersen_verify_batch(leaf.ctx.0, two_to_one.ctx.0, root.as_ptr(), flat.as_ptr(), leaf_len, sib.as_ptr(), paths.as_ptr(),
+                                                 plen, idx.as_ptr(), ok.as_mut_ptr(), idx.len())
+            })?;
+            Ok(ok.into_iter().map(|b| b != 0).collect())
         }
         fn update_impl(&mut self, leaf: &GpuPedersenParams, two_to_one: &GpuPedersenParams, indexes: &[usize], new_leaves: &[Vec<u8>],
                        asserted_new_root: Option<&EdwardsAffine>) -> Result<bool, Error> {
