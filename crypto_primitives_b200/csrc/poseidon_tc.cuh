@@ -175,33 +175,41 @@ template <int NT> struct TcTabShared {
 };
 
 // One output for lane's hash: the GEMM over k-chunks KC0 .. KC0+NT-1 of the table (read through B) against the staged operands
-// 0 .. NT-1, packed, moved to one row per lane through the C buffer, rebuilt and reduced by tc_finish.  m-tile outer, so that only
-// one m-tile's A fragments (4 NT registers) and packed results (8) are live.  Every lane has read the stage when it returns.
+// 0 .. NT-1, packed, moved to one row per lane through the C buffer, rebuilt and reduced by tc_finish.  Both m-tiles at once, so
+// each B fragment is loaded once for two IMMA (DESIGN §4.2).  Every lane has read the stage when it returns.
 template <class F, class B, int NT, int KC0, bool U>
 CPB_D void tc_output(u32* r, const u32* stage, u32* cbuf, const u32* tab, int lane, const u32* y, const u32* pm) {
     const int g = lane >> 2, t = lane & 3;
+    u32 a[2][NT][4];
 #pragma unroll
-    for (int mt = 0; mt < 2; mt++) {
-        u32 a[NT][4];
+    for (int mt = 0; mt < 2; mt++)
 #pragma unroll
         for (int kc = 0; kc < NT; kc++)
-            tc_ldsm_x4(a[kc], stage + (16 * mt + tc_ldsm_row(lane)) * kTcStageStride + 8 * kc + 4 * tc_ldsm_half(lane));
-        u32 pk[2][4];                                   // [C row g / g + 8 of this m-tile][n-tile]
+            tc_ldsm_x4(a[mt][kc], stage + (16 * mt + tc_ldsm_row(lane)) * kTcStageStride + 8 * kc + 4 * tc_ldsm_half(lane));
+    u32 pk[2][2][4];                                    // [m-tile][C row g / g + 8 of it][n-tile]
 #pragma unroll
-        for (int nt = 0; nt < 4; nt++) {
-            u32 c[4] = {0u, 0u, 0u, 0u};
+    for (int nt = 0; nt < 4; nt++) {
+        u32 c[2][4] = {{0u, 0u, 0u, 0u}, {0u, 0u, 0u, 0u}};
 #pragma unroll
-            for (int kc = 0; kc < NT; kc++)
-                tc_mma(c, a[kc], B::ld(tab + tc_tab_word(nt, KC0 + kc, lane, 0, B::kTerms)));
-            pk[0][nt] = c[0] + (c[1] << 8);             // columns 2t, 2t + 1: 16-bit digit 4 nt + t of the row's V
-            pk[1][nt] = c[2] + (c[3] << 8);
+        for (int kc = 0; kc < NT; kc++) {
+            const uint2 b = B::ld(tab + tc_tab_word(nt, KC0 + kc, lane, 0, B::kTerms));   // one load for both m-tiles
+            tc_mma(c[0], a[0][kc], b);
+            tc_mma(c[1], a[1][kc], b);
         }
+#pragma unroll
+        for (int mt = 0; mt < 2; mt++) {
+            pk[mt][0][nt] = c[mt][0] + (c[mt][1] << 8);  // columns 2t, 2t + 1: 16-bit digit 4 nt + t of the row's V
+            pk[mt][1][nt] = c[mt][2] + (c[mt][3] << 8);
+        }
+    }
+#pragma unroll
+    for (int mt = 0; mt < 2; mt++)
 #pragma unroll
         for (int u = 0; u < 2; u++) {
             const int row = 16 * mt + 8 * u + g;
-            *reinterpret_cast<uint4*>(cbuf + 16 * row + 4 * tc_cbuf_chunk(row, t)) = make_uint4(pk[u][0], pk[u][1], pk[u][2], pk[u][3]);
+            *reinterpret_cast<uint4*>(cbuf + 16 * row + 4 * tc_cbuf_chunk(row, t)) =
+                make_uint4(pk[mt][u][0], pk[mt][u][1], pk[mt][u][2], pk[mt][u][3]);
         }
-    }
     __syncwarp();
     u32 h[16];
 #pragma unroll

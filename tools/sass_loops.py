@@ -9,7 +9,7 @@ import subprocess
 import sys
 
 CLASSES = ("IMAD.WIDE", "IMAD.HI", "IMAD.MOV", "IMAD.X", "IMAD.IADD", "IMAD", "IADD3.X", "IADD3", "SEL", "MOV", "HFMA2", "LOP3",
-           "ISETP", "LDG", "LDSM", "LDS", "STS", "IMMA", "STL", "LDL", "BRA")
+           "ISETP", "LDG", "LDSM", "LDS", "STS", "IMMA", "IGMMA", "WARPGROUP", "STL", "LDL", "BRA")
 
 
 def kernels(lib, pat):
