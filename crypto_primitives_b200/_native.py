@@ -17,6 +17,13 @@ vp = C.c_void_p
 
 CPB_OK, CPB_BAD_LENGTH, CPB_BAD_PARAMS, CPB_NOT_POW2, CPB_CUDA_ERROR, CPB_NO_DEVICE, CPB_UNSUPPORTED, CPB_NULL_POINTER, CPB_INTERNAL_ERROR, CPB_NCCL_ERROR = range(10)
 
+class SpongeMode(C.Structure):
+    """cpb_sponge_mode (DuplexSpongeMode): squeezing 0 = Absorbing{index}, 1 = Squeezing{index}."""
+    _fields_ = [("squeezing", C.c_int), ("index", C.c_size_t)]
+
+
+modep = C.POINTER(SpongeMode)
+
 # name -> (restype, argtypes); mirrors include/cpb200.h one to one (tests/test_abi.py checks it).
 SIGNATURES = {
     "cpb_last_error": (C.c_char_p, []),
@@ -56,6 +63,12 @@ SIGNATURES = {
     "cpb_merkle_poseidon_verify_ragged_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp, vp, C.c_size_t, vp]),
     "cpb_poseidon_compress_batch": (C.c_int, [vp, u64p, u64p, C.c_size_t]),
     "cpb_poseidon_compress_batch_dev": (C.c_int, [vp, vp, vp, C.c_size_t, vp]),
+    "cpb_poseidon_duplex_absorb": (C.c_int, [vp, u64p, modep, u64p, C.c_size_t, C.c_size_t]),
+    "cpb_poseidon_duplex_absorb_dev": (C.c_int, [vp, vp, modep, vp, C.c_size_t, C.c_size_t, vp]),
+    "cpb_poseidon_duplex_absorb_bytes": (C.c_int, [vp, u64p, modep, u8p, C.c_size_t, C.c_size_t, C.c_size_t]),
+    "cpb_poseidon_duplex_absorb_bytes_dev": (C.c_int, [vp, vp, modep, vp, C.c_size_t, C.c_size_t, C.c_size_t, vp]),
+    "cpb_poseidon_duplex_squeeze": (C.c_int, [vp, u64p, modep, u64p, C.c_size_t, C.c_int, C.c_size_t]),
+    "cpb_poseidon_duplex_squeeze_dev": (C.c_int, [vp, vp, modep, vp, C.c_size_t, C.c_int, C.c_size_t, vp]),
     "cpb_merkle_poseidon_build": (C.c_int, [vp, vp, u64p, C.c_size_t, C.c_size_t, u64p, u64p]),
     "cpb_merkle_poseidon_build_dev": (C.c_int, [vp, vp, vp, C.c_size_t, C.c_size_t, vp, vp, vp]),
     "cpb_merkle_poseidon_from_digests": (C.c_int, [vp, u64p, C.c_size_t, u64p]),

@@ -112,6 +112,10 @@ CPB_POS_WIDTHS(CPB_POS_EXTERN_RAGGED, Bls12_381_Fr)
 CPB_POS_WIDTHS(CPB_POS_EXTERN_RAGGED, Bn254_Fr)
 CPB_POS_WIDTHS(CPB_POS_EXTERN_RAGGED, Jubjub_Fr)
 CPB_POS_WIDTHS(CPB_POS_EXTERN_RAGGED, Bls12_377_Fr)
+CPB_POS_WIDTHS(CPB_POS_EXTERN_DUPLEX, Bls12_381_Fr)
+CPB_POS_WIDTHS(CPB_POS_EXTERN_DUPLEX, Bn254_Fr)
+CPB_POS_WIDTHS(CPB_POS_EXTERN_DUPLEX, Jubjub_Fr)
+CPB_POS_WIDTHS(CPB_POS_EXTERN_DUPLEX, Bls12_377_Fr)
 CPB_POS_EXTERN_TEAM(Bls12_381_Fr)
 CPB_POS_EXTERN_TEAM(Bn254_Fr)
 CPB_POS_EXTERN_TEAM(Jubjub_Fr)
@@ -1134,6 +1138,130 @@ cpb_status cpb_merkle_poseidon_verify_ragged_batch(cpb_poseidon_ctx* leaf, cpb_p
     CPB_CUDA(cudaStreamSynchronize(st));
     return CPB_OK;
     });
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------ batched duplex sponges
+namespace {
+
+constexpr size_t kDuplexMaxBytes = (size_t)1 << 62;      // every device offset of a call stays far inside a long
+
+bool fits(size_t a, size_t b, size_t c = 1) {
+    if (b && a > kDuplexMaxBytes / b) return false;
+    return a * b <= kDuplexMaxBytes / c;
+}
+
+// The checks that need no context, in the header's order: the mode, the sizes, then the buffers.
+cpb_status duplex_check_mode(const cpb_sponge_mode* mode) {
+    if (!mode) return fail(CPB_NULL_POINTER, "null mode");
+    if (mode->squeezing != 0 && mode->squeezing != 1) return fail(CPB_BAD_PARAMS, "mode.squeezing must be 0 or 1 (got %d)", mode->squeezing);
+    return CPB_OK;
+}
+cpb_status duplex_check_ctx(const cpb_poseidon_ctx* c, const cpb_sponge_mode* mode) {
+    CPB_TRY(check_ctx(c));
+    if (!duplex_mode_valid(mode->squeezing, mode->index, c->dev.rate))
+        return fail(CPB_BAD_PARAMS, "mode.index %zu exceeds the rate %d", mode->index, c->dev.rate);
+    return CPB_OK;
+}
+
+cpb_status launch_duplex(cpb_poseidon_ctx* c, u32* states, const DuplexOp& op, size_t n, cudaStream_t st) {
+    CPB_FOR_FIELD(launch_duplex_ft, c, states, op, n, st)
+    return fail(CPB_UNSUPPORTED, "state width t=%d is not built (this library: t = 2..9)", c->dev.t);
+}
+
+// One call on the whole batch.  `in_bytes` / `out_bytes`: the host form's copies of op.in or op.bytes and of op.out (host == true:
+// states and every buffer of op are host memory, staged through the context's scratch).  n == 0 or an absorb of nothing only
+// advances the mode.
+cpb_status duplex_call(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, DuplexOp op, size_t n, size_t in_bytes,
+                       size_t out_bytes, bool host, cudaStream_t st) {
+    const DuplexPlan p = duplex_plan(op.kind >= kSqueeze, DuplexMode{mode->squeezing, (long)mode->index}, c->dev.rate, op.count);
+    if (!p.noop && n > 0) {
+        op.first = p.permute_first ? 1 : 0;
+        op.start = p.start;
+        op.boundaries = p.boundaries;
+        DeviceGuard g(c->device);
+        if (!host) {
+            CPB_TRY(launch_duplex(c, (u32*)states, op, n, st));
+        } else {
+            std::lock_guard<std::mutex> lk(c->mu);
+            const size_t s_b = n * (size_t)c->dev.t * 32;
+            CPB_TRY(c->s_aux.reserve(s_b));
+            CPB_TRY(c->s_in.reserve(in_bytes ? in_bytes : 32));
+            CPB_TRY(c->s_out.reserve(out_bytes ? out_bytes : 32));
+            CPB_CUDA(cudaMemcpyAsync(c->s_aux.ptr, states, s_b, cudaMemcpyHostToDevice, c->stream));
+            const void* src = op.kind == kAbsorbBytes ? (const void*)op.bytes : (const void*)op.in;
+            if (in_bytes) CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, src, in_bytes, cudaMemcpyHostToDevice, c->stream));
+            u32* host_out = op.out;
+            op.in = (const u32*)c->s_in.ptr;
+            op.bytes = (const unsigned char*)c->s_in.ptr;
+            op.out = (u32*)c->s_out.ptr;
+            CPB_TRY(launch_duplex(c, (u32*)c->s_aux.ptr, op, n, c->stream));
+            CPB_CUDA(cudaMemcpyAsync(states, c->s_aux.ptr, s_b, cudaMemcpyDeviceToHost, c->stream));
+            if (out_bytes) CPB_CUDA(cudaMemcpyAsync(host_out, c->s_out.ptr, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+            CPB_CUDA(cudaStreamSynchronize(c->stream));
+        }
+    }
+    mode->squeezing = p.mode.squeezing;
+    mode->index = (size_t)p.mode.index;
+    return CPB_OK;
+}
+
+cpb_status duplex_absorb(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, const uint64_t* in, size_t k, size_t n, bool host,
+                         void* stream) {
+    CPB_TRY(duplex_check_mode(mode));
+    if (!fits(n, 16 * 32) || !fits(n, k, 32)) return fail(CPB_BAD_LENGTH, "batch too large (n=%zu, k=%zu)", n, k);
+    if (n && (!states || (k && !in))) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(duplex_check_ctx(c, mode));
+    DuplexOp op{kAbsorb, 0, 0, 0, (long)k, (const u32*)in, nullptr, 0, 0, nullptr};
+    return duplex_call(c, states, mode, op, n, n * k * 32, 0, host, (cudaStream_t)stream);
+}
+cpb_status duplex_absorb_bytes(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, const uint8_t* in, size_t len, size_t stride,
+                               size_t n, bool host, void* stream) {
+    CPB_TRY(duplex_check_mode(mode));
+    if (!fits(n, 16 * 32) || len > kDuplexMaxBytes || (n && !fits(n - 1, stride)) || (n && (n - 1) * stride > kDuplexMaxBytes - len))
+        return fail(CPB_BAD_LENGTH, "batch too large (n=%zu, len=%zu, stride=%zu)", n, len, stride);
+    if (n && (!states || (len && !in))) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(duplex_check_ctx(c, mode));
+    DuplexOp op{kAbsorbBytes, 0, 0, 0, duplex_byte_elems((long)len), nullptr, in, (long)len, (long)stride, nullptr};
+    return duplex_call(c, states, mode, op, n, n ? (n - 1) * stride + len : 0, 0, host, (cudaStream_t)stream);
+}
+cpb_status duplex_squeeze(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, uint64_t* out, size_t m, int canonical, size_t n,
+                          bool host, void* stream) {
+    CPB_TRY(duplex_check_mode(mode));
+    if (!fits(n, 16 * 32) || !fits(n, m, 32)) return fail(CPB_BAD_LENGTH, "batch too large (n=%zu, m=%zu)", n, m);
+    if (n && (!states || (m && !out))) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(duplex_check_ctx(c, mode));
+    DuplexOp op{canonical ? kSqueezeCanonical : kSqueeze, 0, 0, 0, (long)m, nullptr, nullptr, 0, 0, (u32*)out};
+    return duplex_call(c, states, mode, op, n, 0, n * m * 32, host, (cudaStream_t)stream);
+}
+
+}  // namespace
+
+extern "C" {
+
+cpb_status cpb_poseidon_duplex_absorb(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, const uint64_t* in, size_t k, size_t n) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_absorb(c, states, mode, in, k, n, true, nullptr); });
+}
+cpb_status cpb_poseidon_duplex_absorb_dev(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, const uint64_t* in, size_t k,
+                                          size_t n, void* stream) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_absorb(c, states, mode, in, k, n, false, stream); });
+}
+cpb_status cpb_poseidon_duplex_absorb_bytes(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, const uint8_t* in, size_t len,
+                                            size_t stride, size_t n) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_absorb_bytes(c, states, mode, in, len, stride, n, true, nullptr); });
+}
+cpb_status cpb_poseidon_duplex_absorb_bytes_dev(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, const uint8_t* in,
+                                                size_t len, size_t stride, size_t n, void* stream) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_absorb_bytes(c, states, mode, in, len, stride, n, false, stream); });
+}
+cpb_status cpb_poseidon_duplex_squeeze(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, uint64_t* out, size_t m, int canonical,
+                                       size_t n) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_squeeze(c, states, mode, out, m, canonical, n, true, nullptr); });
+}
+cpb_status cpb_poseidon_duplex_squeeze_dev(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, uint64_t* out, size_t m,
+                                           int canonical, size_t n, void* stream) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_squeeze(c, states, mode, out, m, canonical, n, false, stream); });
 }
 
 }  // extern "C"

@@ -6,6 +6,7 @@
 
 #include "common.cuh"
 #include "poseidon.cuh"
+#include "poseidon_duplex.cuh"
 #include "poseidon_host.hpp"
 #include "poseidon_team.cuh"
 
@@ -375,6 +376,33 @@ cpb_status launch_verify_ragged_ft(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* nod
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Batched duplex sponges (poseidon_duplex.cuh): one sponge per thread, grid-stride; states (n, T) elements updated in place.
+// The state is arbitrary, so the permutation takes no PermuteHint.
+// ---------------------------------------------------------------------------------------------------------------
+template <class F, int T>
+__global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
+k_poseidon_duplex(PoseidonDev P, const u32* __restrict__ consts, u32* __restrict__ states, DuplexOp op, long n) {
+    extern __shared__ __align__(16) u32 cs[];
+    __shared__ __align__(8) unsigned long long mbar;
+    tma_stage_to_smem(cs, consts, (unsigned)P.n_elems * 32u, &mbar);
+    const u32* ct = cs + (int)threadIdx.x * P.zero;
+    u32 pm[8];
+    ld_elem(pm, ct + 8 * P.off_mod);
+    const long stride = (long)gridDim.x * blockDim.x;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) pos_duplex<F, T>(states + 8 * T * i, op, i, P, ct, pm);
+}
+
+template <class F, int T>
+cpb_status launch_duplex_ft(cpb_poseidon_ctx* c, u32* states, const DuplexOp& op, size_t n, cudaStream_t st) {
+    size_t smem = (size_t)c->dev.n_elems * 32;
+    int grid = 1;
+    CPB_TRY(grid_for(k_poseidon_duplex<F, T>, smem, c->sms, (long)n, grid));
+    k_poseidon_duplex<F, T><<<grid, kBlock, smem, st>>>(c->dev, c->d_consts, states, op, (long)n);
+    CPB_CUDA(cudaGetLastError());
+    return CPB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Tree-top kernel: ALL the small levels of a Merkle (sub)tree in one launch, four warps per 32 hashes
 // (poseidon_team.cuh), and -- on a multi-GPU build -- the exchange of the subtree roots over NVLink peer memory and
 // the replicated top levels in the same kernel.  t = 3, capacity 1 (poseidon::TwoToOneCRH) only.
@@ -623,6 +651,9 @@ cpb_status merkle_build_streams(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, 
 #define CPB_POS_EXTERN_DIGESTS(F, T)                                                                                     \
     extern template cpb_status launch_verify_digests_ft<F, T>(cpb_poseidon_ctx*, const u32*, const u32*, const u32*, const u32*, \
                                                               int, const unsigned long long*, unsigned char*, size_t, cudaStream_t);
+// the duplex kernels (poseidon_duplex_<field>.cu), likewise in units of their own
+#define CPB_POS_INSTANTIATE_DUPLEX(F, T) template cpb_status launch_duplex_ft<F, T>(cpb_poseidon_ctx*, u32*, const DuplexOp&, size_t, cudaStream_t);
+#define CPB_POS_EXTERN_DUPLEX(F, T) extern template cpb_status launch_duplex_ft<F, T>(cpb_poseidon_ctx*, u32*, const DuplexOp&, size_t, cudaStream_t);
 #define CPB_POS_INSTANTIATE_TEAM(F) template cpb_status launch_tree_top_f<F>(cpb_poseidon_ctx*, TopJob, cudaStream_t);
 #define CPB_POS_EXTERN_TEAM(F) extern template cpb_status launch_tree_top_f<F>(cpb_poseidon_ctx*, TopJob, cudaStream_t);
 #define CPB_POS_EXTERN(F, T)                                                                                             \

@@ -103,15 +103,26 @@ def get_default_poseidon_parameters(field: Field, rate: int, optimized_for_weigh
 FULL = "Full"        # FieldElementSize::Full; an int is FieldElementSize::Truncated(bits) (R/sponge/mod.rs:24-36)
 
 
+def _c_mode(mode) -> "N.SpongeMode":
+    kind, idx = mode
+    if kind not in ("Absorbing", "Squeezing"):
+        raise ValueError(f"unknown sponge mode {kind!r}")
+    return N.SpongeMode(int(kind == "Squeezing"), int(idx))
+
+
+def _py_mode(m) -> tuple:
+    return ("Squeezing" if m.squeezing else "Absorbing", int(m.index))
+
+
 class PoseidonSponge:
     """Duplex sponge over the GPU permutation -- host mirror of PoseidonSponge<F> (R/sponge/poseidon/mod.rs:47-63):
     CryptographicSponge::{new, absorb, squeeze_bytes, squeeze_bits, squeeze_field_elements} (mod.rs:220-321) and
-    FieldBasedCryptographicSponge::squeeze_native_field_elements (mod.rs:323-345), with the same mode bookkeeping
-    (absorb_internal / squeeze_internal, mod.rs:124-186), `fork` (R/sponge/mod.rs:145-153), the sized squeezes
-    (R/sponge/mod.rs:57-96,170-187) and SpongeExt::{from_state, into_state} (mod.rs:347-370).  `absorb` takes native
-    field elements as (k, 4) Montgomery limbs or any value sponge/absorb.py can encode (R/sponge/absorb.rs).  Every
-    permutation is one GPU call of batch size 1: correct but slow -- a single transcript is sequential by nature; for
-    many independent sponges use `absorb_squeeze_batch`."""
+    FieldBasedCryptographicSponge::squeeze_native_field_elements (mod.rs:323-345), `fork` (R/sponge/mod.rs:145-153), the sized
+    squeezes (R/sponge/mod.rs:57-96,170-187) and SpongeExt::{from_state, into_state} (mod.rs:347-370).  `absorb` takes native
+    field elements as (k, 4) Montgomery limbs or any value sponge/absorb.py can encode (R/sponge/absorb.rs).  It is the n = 1 case
+    of the batched duplex (cpb_poseidon_duplex_*, host form): one library call per absorb or squeeze, which runs every permutation
+    that call needs and the reference's mode bookkeeping (absorb_internal / squeeze_internal, mod.rs:124-186) on the GPU.  For many
+    sponges running the same script use PoseidonSpongeBatch."""
 
     def __init__(self, parameters: PoseidonConfig, device: int = 0):
         self.parameters = parameters
@@ -124,49 +135,12 @@ class PoseidonSponge:
     def new(cls, parameters: PoseidonConfig, device: int = 0):
         return cls(parameters, device)
 
-    # -- internals
-    def _permute(self):
-        out = np.empty_like(self.state)
-        N.check(N.lib.cpb_poseidon_permute_batch(self.parameters.context(self.device), self.state.ctypes.data_as(N.u64p),
-                                                 out.ctypes.data_as(N.u64p), 1))
-        self.state = out
-
-    def _add(self, lane: int, elem: np.ndarray):
-        f = self.parameters.field
-        a, b = f.to_ints(self.state[lane])[0], f.to_ints(elem)[0]
-        self.state[lane] = f.elements([(a + b) % f.modulus])[0]
-
-    def _absorb_internal(self, rate_start: int, elems: np.ndarray):           # mod.rs:124-153
-        c = self.parameters
-        rem = elems
-        while True:
-            if rate_start + len(rem) <= c.rate:
-                for i, e in enumerate(rem):
-                    self._add(c.capacity + i + rate_start, e)
-                self.mode = ("Absorbing", rate_start + len(rem))
-                return
-            k = c.rate - rate_start
-            for i, e in enumerate(rem[:k]):
-                self._add(c.capacity + i + rate_start, e)
-            self._permute()
-            rem = rem[k:]
-            rate_start = 0
-
-    def _squeeze_internal(self, rate_start: int, n_out: int) -> np.ndarray:  # mod.rs:156-186
-        c = self.parameters
-        out = []
-        rem = n_out
-        while True:
-            if rate_start + rem <= c.rate:
-                out.extend(self.state[c.capacity + rate_start: c.capacity + rate_start + rem])
-                self.mode = ("Squeezing", rate_start + rem)
-                return np.array(out, dtype=np.uint64).reshape(-1, 4)
-            k = c.rate - rate_start
-            out.extend(self.state[c.capacity + rate_start: c.capacity + rate_start + k])
-            rem -= k
-            if rem != 0:
-                self._permute()
-            rate_start = 0
+    # -- internals: one duplex call of batch size 1 on the host-form C-ABI
+    def _call(self, fn, *args):
+        st = np.ascontiguousarray(self.state, dtype=np.uint64).copy()
+        m = _c_mode(self.mode)
+        N.check(fn(self.parameters.context(self.device), st.ctypes.data_as(N.u64p), C.byref(m), *args, 1))
+        self.state, self.mode = st, _py_mode(m)
 
     # -- public surface
     def clone(self) -> "PoseidonSponge":
@@ -191,31 +165,21 @@ class PoseidonSponge:
 
     def absorb(self, elems):
         """elems: (k, 4) Montgomery limbs (or a single (4,) element), or any absorbable of sponge/absorb.py."""
+        if isinstance(elems, (bytes, bytearray)):                              # the [u8] rule, encoded on the device
+            b = np.frombuffer(bytes(elems), dtype=np.uint8)
+            self._call(N.lib.cpb_poseidon_duplex_absorb_bytes, b.ctypes.data_as(N.u8p) if len(b) else None, len(b), 0)
+            return
         if isinstance(elems, np.ndarray):
-            e = np.asarray(elems, dtype=np.uint64).reshape(-1, 4)
+            e = np.ascontiguousarray(elems, dtype=np.uint64).reshape(-1, 4)
         else:
             from .absorb import to_sponge_field_elements
-            e = to_sponge_field_elements(elems, self.parameters.field)
-        if e.shape[0] == 0:
-            return
-        kind, idx = self.mode
-        if kind == "Absorbing":
-            if idx == self.parameters.rate:
-                self._permute()
-                idx = 0
-            self._absorb_internal(idx, e)
-        else:
-            self._absorb_internal(0, e)
+            e = np.ascontiguousarray(to_sponge_field_elements(elems, self.parameters.field))
+        self._call(N.lib.cpb_poseidon_duplex_absorb, e.ctypes.data_as(N.u64p), e.shape[0])
 
     def squeeze_native_field_elements(self, num_elements: int) -> np.ndarray:
-        kind, idx = self.mode
-        if kind == "Absorbing":
-            self._permute()
-            return self._squeeze_internal(0, num_elements)
-        if idx == self.parameters.rate:
-            self._permute()
-            idx = 0
-        return self._squeeze_internal(idx, num_elements)
+        out = np.zeros((max(num_elements, 1), 4), dtype=np.uint64)
+        self._call(N.lib.cpb_poseidon_duplex_squeeze, out.ctypes.data_as(N.u64p), num_elements, 0)
+        return out[:num_elements]
 
     def squeeze_field_elements(self, num_elements: int, field: Field | None = None) -> np.ndarray:
         """mod.rs:309-320: the native fast path, else `num_elements` Full-size elements of `field`."""
@@ -271,6 +235,207 @@ class PoseidonSponge:
         for v in f.to_ints(self.squeeze_native_field_elements(n)):
             bits.extend(bool((v >> i) & 1) for i in range(usable))
         return bits[:num_bits]
+
+
+class PoseidonSpongeBatch:
+    """n independent PoseidonSponge over one PoseidonConfig that run the same script: the states are a torch CUDA int64 tensor
+    (n, t, 4) of Montgomery limbs on `device`, and the batch has one DuplexSpongeMode.  Every absorb or squeeze is one call of the
+    _dev C-ABI (cpb_poseidon_duplex_*) on the current torch stream, which runs every permutation of the call for all n sponges in
+    one kernel launch.  Results are torch tensors on the device; sponge(i) continues item i as an independent PoseidonSponge."""
+
+    def __init__(self, parameters: PoseidonConfig, n: int, device=None):
+        import torch
+        self.parameters = parameters
+        self.n = int(n)
+        self.device = _cuda_device(device)
+        t = parameters.rate + parameters.capacity
+        self.states = torch.zeros((self.n, t, 4), dtype=torch.int64, device=self.device)
+        self._mode = N.SpongeMode(0, 0)
+
+    # -- state
+    @property
+    def mode(self) -> tuple:
+        return _py_mode(self._mode)
+
+    @classmethod
+    def from_states(cls, states, mode, parameters: PoseidonConfig, device=None) -> "PoseidonSpongeBatch":
+        """SpongeExt::from_state for the batch: states (n, t, 4) Montgomery limbs (torch or numpy), mode ("Absorbing"|"Squeezing", index)."""
+        st = _as_i64(states, _cuda_device(device))
+        b = cls(parameters, st.shape[0], st.device)
+        t = parameters.rate + parameters.capacity
+        if tuple(st.shape[1:]) != (t, 4):
+            raise ValueError(f"states must be (n, {t}, 4)")
+        b.states = st.contiguous().clone()
+        b._mode = _c_mode(mode)
+        return b
+
+    def into_states(self):
+        return self.states, self.mode
+
+    def clone(self) -> "PoseidonSpongeBatch":
+        c = PoseidonSpongeBatch.__new__(PoseidonSpongeBatch)
+        c.parameters, c.n, c.device = self.parameters, self.n, self.device
+        c.states = self.states.clone()
+        c._mode = N.SpongeMode(self._mode.squeezing, self._mode.index)
+        return c
+
+    def sponge(self, i: int) -> PoseidonSponge:
+        """Item i as an independent PoseidonSponge (host state)."""
+        st = self.states[i].cpu().numpy().view(np.uint64)
+        return PoseidonSponge.from_state((st, self.mode), self.parameters, self.device.index)
+
+    # -- internals
+    def _stream(self):
+        import torch
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def _ctx(self):
+        return self.parameters.context(self.device.index)
+
+    # -- absorb
+    def absorb(self, x):
+        """x: (n, k, 4) native elements (torch or numpy limbs); (n, L) uint8 byte strings, one per sponge; one `bytes` value for every
+        sponge; or a sequence of n absorbables (sponge/absorb.py), one per sponge, that encode to the same number of elements."""
+        import torch
+        if isinstance(x, (bytes, bytearray)):
+            b = torch.tensor(list(x), dtype=torch.uint8, device=self.device)
+            N.check(N.lib.cpb_poseidon_duplex_absorb_bytes_dev(self._ctx(), self.states.data_ptr(), C.byref(self._mode),
+                                                               b.data_ptr() if len(x) else None, len(x), 0, self.n, self._stream()))
+            return
+        if isinstance(x, (np.ndarray, torch.Tensor)) and x.dtype in (np.uint8, torch.uint8):
+            b = torch.as_tensor(x).to(self.device).contiguous()
+            if b.ndim != 2 or b.shape[0] != self.n:
+                raise ValueError(f"byte strings must be (n={self.n}, L) uint8")
+            L = b.shape[1]
+            N.check(N.lib.cpb_poseidon_duplex_absorb_bytes_dev(self._ctx(), self.states.data_ptr(), C.byref(self._mode),
+                                                               b.data_ptr() if L else None, L, L, self.n, self._stream()))
+            return
+        if isinstance(x, (np.ndarray, torch.Tensor)):
+            e = _as_i64(x, self.device)
+        else:
+            from .absorb import to_sponge_field_elements
+            items = list(x)
+            if len(items) != self.n:
+                raise ValueError(f"expected {self.n} absorbables, one per sponge (got {len(items)})")
+            enc = [to_sponge_field_elements(v, self.parameters.field) for v in items]
+            if len({a.shape[0] for a in enc}) > 1:
+                raise ValueError("the items encode to different numbers of field elements; a batch absorbs one length")
+            e = _as_i64(np.stack(enc) if enc else np.zeros((0, 0, 4), dtype=np.uint64), self.device)
+        e = e.reshape(self.n, -1, 4).contiguous()
+        k = e.shape[1]
+        N.check(N.lib.cpb_poseidon_duplex_absorb_dev(self._ctx(), self.states.data_ptr(), C.byref(self._mode),
+                                                     e.data_ptr() if k else None, k, self.n, self._stream()))
+
+    def fork(self, domain) -> "PoseidonSpongeBatch":
+        """R/sponge/mod.rs:145-153 for every sponge: clone, then absorb the byte string usize(len(domain)) || domain.  domain: one
+        `bytes` value for every sponge or (n, L) uint8, one per sponge."""
+        import torch
+        new = self.clone()
+        if isinstance(domain, (bytes, bytearray)):
+            new.absorb(len(domain).to_bytes(8, "little") + bytes(domain))
+            return new
+        d = torch.as_tensor(domain).to(self.device, torch.uint8)
+        if d.ndim != 2 or d.shape[0] != self.n:
+            raise ValueError(f"domains must be (n={self.n}, L) uint8")
+        prefix = torch.tensor(list(d.shape[1].to_bytes(8, "little")), dtype=torch.uint8, device=self.device).expand(self.n, 8)
+        new.absorb(torch.cat([prefix, d], dim=1))
+        return new
+
+    # -- squeeze
+    def _squeeze(self, m: int, canonical: bool):
+        import torch
+        out = torch.empty((self.n, m, 4), dtype=torch.int64, device=self.device)
+        N.check(N.lib.cpb_poseidon_duplex_squeeze_dev(self._ctx(), self.states.data_ptr(), C.byref(self._mode),
+                                                      out.data_ptr() if out.numel() else None, m, int(canonical), self.n,
+                                                      self._stream()))
+        return out
+
+    def squeeze_native_field_elements(self, num_elements: int):
+        """(n, num_elements, 4) Montgomery limbs (torch int64 on the device)."""
+        return self._squeeze(num_elements, False)
+
+    def squeeze_canonical(self, num_elements: int):
+        """squeeze_native_field_elements as canonical integers: (n, num_elements, 4) little-endian limbs."""
+        return self._squeeze(num_elements, True)
+
+    def squeeze_bytes(self, num_bytes: int):
+        """mod.rs:259-274: (n, num_bytes) uint8."""
+        usable = (self.parameters.field.modulus_bit_size - 1) // 8
+        m = (num_bytes + usable - 1) // usable
+        c = self.squeeze_canonical(m).view(__import__("torch").uint8).reshape(self.n, m, 32)
+        return c[:, :, :usable].reshape(self.n, m * usable)[:, :num_bytes]
+
+    def squeeze_bits(self, num_bits: int):
+        """mod.rs:276-291: (n, num_bits) bool."""
+        import torch
+        usable = self.parameters.field.modulus_bit_size - 1
+        m = (num_bits + usable - 1) // usable
+        c = self.squeeze_canonical(m).view(torch.uint8).reshape(self.n, m, 32)
+        bits = (c[..., None] >> torch.arange(8, device=self.device, dtype=torch.uint8)) & 1
+        return bits.reshape(self.n, m, 256)[:, :, :usable].reshape(self.n, m * usable)[:, :num_bits].bool()
+
+    def squeeze_field_elements(self, num_elements: int, field: Field | None = None):
+        """mod.rs:309-320: (n, num_elements, 4) Montgomery limbs of `field` (default: native)."""
+        if field is None or field.id == self.parameters.field.id:
+            return self.squeeze_native_field_elements(num_elements)
+        return self.squeeze_field_elements_with_sizes([FULL] * num_elements, field)
+
+    def squeeze_native_field_elements_with_sizes(self, sizes):
+        return self.squeeze_field_elements_with_sizes(sizes, None)
+
+    def squeeze_field_elements_with_sizes(self, sizes, field: Field | None = None):
+        """mod.rs:291-307 over R/sponge/mod.rs:57-96 (PoseidonSponge.squeeze_field_elements_with_sizes for every sponge):
+        (n, len(sizes), 4) Montgomery limbs of `field`, converted on the device."""
+        import torch
+        native = self.parameters.field
+        field = native if field is None else field
+        sizes = list(sizes)
+        if field.modulus == native.modulus and all(s == FULL for s in sizes):
+            return self.squeeze_native_field_elements(len(sizes))
+        if not sizes:
+            return torch.zeros((self.n, 0, 4), dtype=torch.int64, device=self.device)
+        widths = []
+        for s in sizes:
+            if s == FULL:
+                widths.append(field.modulus_bit_size - 1)
+            elif s > field.modulus_bit_size:
+                raise ValueError("num_bits is greater than the capacity of the field.")   # R/sponge/mod.rs:39-42
+            else:
+                widths.append(int(s))
+        bits = self.squeeze_bits(sum(widths))
+        S = len(sizes)
+        padded = torch.zeros((self.n, S, 256), dtype=torch.int64, device=self.device)
+        pos = 0
+        for j, w in enumerate(widths):
+            padded[:, j, :w] = bits[:, pos:pos + w]
+            pos += w
+        shifts = torch.arange(64, device=self.device, dtype=torch.int64)
+        limbs = (padded.view(self.n, S, 4, 64) << shifts).sum(-1).contiguous()       # disjoint bits: the sum is the OR
+        N.check(N.lib.cpb_field_to_montgomery_dev(field.id, self.device.index, limbs.data_ptr(), limbs.data_ptr(), self.n * S,
+                                                  self._stream()))
+        return limbs
+
+
+def _cuda_device(device):
+    import torch
+    if device is None:
+        return torch.device("cuda", torch.cuda.current_device())
+    if isinstance(device, int):
+        return torch.device("cuda", device)
+    d = torch.device(device)
+    if d.type != "cuda":
+        raise ValueError("PoseidonSpongeBatch keeps its states on a CUDA device")
+    return torch.device("cuda", torch.cuda.current_device() if d.index is None else d.index)
+
+
+def _as_i64(x, device):
+    """Montgomery limbs (numpy uint64/int64 or torch int64) -> contiguous torch int64 on `device`."""
+    import torch
+    if isinstance(x, np.ndarray):
+        x = torch.from_numpy(np.ascontiguousarray(x, dtype=np.uint64).view(np.int64))
+    if x.dtype != torch.int64:
+        raise TypeError("field elements are int64 (or uint64) limbs")
+    return x.to(device).contiguous()
 
 
 def absorb_squeeze_batch(parameters: PoseidonConfig, inputs, num_squeeze: int, device: int = 0) -> np.ndarray:

@@ -77,7 +77,8 @@ typedef struct cpb_multi cpb_multi;         /* a group of GPUs driven by one pro
 const char* cpb_last_error(void);
 
 /* ABI revision of this header: bumped when entry points or status codes are added (2 = CPB_INTERNAL_ERROR, cpb_abi_version; 3 = _dev field conversion, host pinning, launch count, multi-GPU build, CPB_NCCL_ERROR, wire formats; 4 = ragged Poseidon batches: CRH, sponge, Merkle build and path verification over inputs of different lengths; 5 = Merkle update and
- * check_update of Poseidon-node trees, in place on device arrays or over host arrays). */
+ * check_update of Poseidon-node trees, in place on device arrays or over host arrays; later additions under 5 are additive: Merkle path verification of the Pedersen
+ * trees, batched duplex sponges with the cpb_sponge_mode type). */
 #define CPB_ABI_VERSION 5
 int cpb_abi_version(void);
 int cpb_version(void);
@@ -147,6 +148,40 @@ cpb_status cpb_poseidon_sponge_batch_dev(cpb_poseidon_ctx* ctx, const uint64_t* 
 cpb_status cpb_poseidon_compress_batch(cpb_poseidon_ctx* ctx, const uint64_t* pairs, uint64_t* out, size_t n);
 cpb_status cpb_poseidon_compress_batch_dev(cpb_poseidon_ctx* ctx, const uint64_t* pairs, uint64_t* out, size_t n,
                                            void* stream);
+
+/* ---- Batched duplex sponges -------------------------------------------------------------------------------------- */
+/* DuplexSpongeMode (R/sponge/mod.rs): squeezing == 0 is Absorbing{next_absorb_index = index}, 1 is Squeezing{next_squeeze_index}. */
+typedef struct cpb_sponge_mode {
+    int squeezing;
+    size_t index;
+} cpb_sponge_mode;
+/* n independent PoseidonSponge<F> over one context that share one mode: states (n x t elements, Montgomery, the layout of
+ * cpb_poseidon_permute_batch) are updated in place and *mode (host memory) is read and advanced by every call.  Each call applies
+ * the same operation to every sponge with the mode rules of the reference (R/sponge/poseidon/mod.rs:124-186, 236-257, 323-345):
+ *   absorb         k native elements per sponge from in + 4*k*i; k == 0 does nothing;
+ *   absorb_bytes   the byte string of `len` bytes at in + stride*i (stride 0: one string for every sponge), encoded as
+ *                  Absorb for [u8] (R/sponge/absorb.rs:137-141): an 8-byte little-endian length, then the bytes, in
+ *                  31-byte little-endian chunks, i.e. ceil((len + 8) / 31) elements;
+ *   squeeze        squeeze_native_field_elements(m) to out + 4*m*i, as Montgomery limbs or (canonical != 0) as canonical
+ *                  integers; m == 0 still permutes from Absorbing mode.
+ * Argument checks, before any device work, in this order: mode == NULL -> CPB_NULL_POINTER, mode->squeezing not 0 or 1 ->
+ * CPB_BAD_PARAMS; sizes beyond 2^62 bytes -> CPB_BAD_LENGTH; a buffer the call reads or writes (n > 0) NULL -> CPB_NULL_POINTER;
+ * ctx NULL -> CPB_NULL_POINTER; mode->index > rate -> CPB_BAD_PARAMS.  n == 0 advances the mode and launches nothing: the mode
+ * belongs to the batch.  On an error the mode is unchanged.
+ * Host forms: host arrays, copied in and out.  _dev forms: device arrays, enqueued on `stream` without host synchronisation
+ * (CUDA-graph capturable). */
+cpb_status cpb_poseidon_duplex_absorb(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* mode, const uint64_t* in, size_t k,
+                                      size_t n);
+cpb_status cpb_poseidon_duplex_absorb_dev(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* mode, const uint64_t* in, size_t k,
+                                          size_t n, void* stream);
+cpb_status cpb_poseidon_duplex_absorb_bytes(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* mode, const uint8_t* in, size_t len,
+                                            size_t stride, size_t n);
+cpb_status cpb_poseidon_duplex_absorb_bytes_dev(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* mode, const uint8_t* in,
+                                                size_t len, size_t stride, size_t n, void* stream);
+cpb_status cpb_poseidon_duplex_squeeze(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* mode, uint64_t* out, size_t m,
+                                       int canonical, size_t n);
+cpb_status cpb_poseidon_duplex_squeeze_dev(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* mode, uint64_t* out, size_t m,
+                                           int canonical, size_t n, void* stream);
 
 /* ---- Merkle tree, field leaves ---------------------------------------------------------- */
 /* MerkleTree::new (R/merkle_tree/mod.rs:411-422) for Config{Leaf=[F], LeafDigest=InnerDigest=F,

@@ -132,6 +132,47 @@ struct TwoToOneCRH {
     }
 };
 
+// n PoseidonSponge<F> over one Config that share one DuplexSpongeMode (R/sponge/poseidon/mod.rs:47-63, 124-186, 220-345): every
+// call applies the same absorb or squeeze to all n sponges with per-sponge data, one cpb_poseidon_duplex_* call for the batch.
+// States are host memory (n x t elements, Montgomery); the Config must outlive the batch.  One transcript is n = 1.
+class PoseidonSpongeBatch {
+public:
+    PoseidonSpongeBatch(const Config& p, size_t n)
+        : p_(&p), n_(n), states_(n * (size_t)(p.rate + p.capacity), Fe{0, 0, 0, 0}), mode_{0, 0} {}
+
+    // absorb k native elements per sponge: elems is n x k, sponge i's at elems[i * k ..]
+    void absorb(const std::vector<Fe>& elems) {
+        const size_t k = n_ ? elems.size() / n_ : 0;
+        if (n_ && elems.size() != n_ * k) throw Error(CPB_BAD_LENGTH, "absorb: elems.size() is not a multiple of n");
+        check(cpb_poseidon_duplex_absorb(p_->ctx(), data(), &mode_, k ? elems[0].data() : nullptr, k, n_));
+    }
+    // absorb one byte string per sponge (the [u8] rule, R/sponge/absorb.rs:137-141): sponge i's `len` bytes at bytes[i * stride ..];
+    // stride 0 gives every sponge the same string
+    void absorb_bytes(const std::vector<uint8_t>& bytes, size_t len, size_t stride) {
+        if (n_ && len && bytes.size() < (n_ - 1) * stride + len) throw Error(CPB_BAD_LENGTH, "absorb_bytes: buffer too short");
+        check(cpb_poseidon_duplex_absorb_bytes(p_->ctx(), data(), &mode_, len ? bytes.data() : nullptr, len, stride, n_));
+    }
+    // squeeze_native_field_elements(m) of every sponge: n x m Montgomery elements, or canonical integers
+    std::vector<Fe> squeeze_native_field_elements(size_t m) { return squeeze(m, false); }
+    std::vector<Fe> squeeze_canonical(size_t m) { return squeeze(m, true); }
+
+    size_t size() const { return n_; }
+    const std::vector<Fe>& states() const { return states_; }    // sponge i's state at [i * t ..]
+    cpb_sponge_mode mode() const { return mode_; }
+
+private:
+    std::vector<Fe> squeeze(size_t m, bool canonical) {
+        std::vector<Fe> out(n_ * m);
+        check(cpb_poseidon_duplex_squeeze(p_->ctx(), data(), &mode_, out.empty() ? nullptr : out[0].data(), m, canonical ? 1 : 0, n_));
+        return out;
+    }
+    uint64_t* data() { return states_.empty() ? nullptr : states_[0].data(); }
+    const Config* p_;
+    size_t n_;
+    std::vector<Fe> states_;
+    cpb_sponge_mode mode_;
+};
+
 }  // namespace poseidon
 
 namespace pedersen {

@@ -2,13 +2,15 @@
 //!
 //! SOURCE ONLY (not compiled in this repository: the image has no Rust toolchain).  It shows exactly what a
 //! maintainer binds: the raw `extern "C"` block mirrors `include/cpb200.h`; the wrappers implement
-//! `CRHScheme` / `TwoToOneCRHScheme` (R/crh/mod.rs:18-51) for Poseidon and a `GpuMerkleTree` with the
+//! `CRHScheme` / `TwoToOneCRHScheme` (R/crh/mod.rs:18-51) for Poseidon, `CryptographicSponge` + `FieldBasedCryptographicSponge`
+//! (R/sponge/mod.rs) for `GpuPoseidonSponge`, and a `GpuMerkleTree` with the
 //! reference's public method set (R/merkle_tree/mod.rs:397-533).  `ark-crypto-primitives` itself forbids
 //! `unsafe` (R/lib.rs:9), hence a sibling crate.
 use ark_crypto_primitives::crh::{CRHScheme, TwoToOneCRHScheme};
 use ark_crypto_primitives::sponge::poseidon::PoseidonConfig;
+use ark_crypto_primitives::sponge::{Absorb, CryptographicSponge, FieldBasedCryptographicSponge, FieldElementSize};
 use ark_crypto_primitives::Error;
-use ark_ff::{BigInt, Fp256, MontBackend, MontConfig, PrimeField};
+use ark_ff::{BigInt, BigInteger, Fp256, MontBackend, MontConfig, PrimeField};
 use ark_std::{borrow::Borrow, marker::PhantomData, rand::Rng, sync::Arc};
 use std::os::raw::{c_char, c_int};
 
@@ -35,6 +37,13 @@ extern "C" {
     fn cpb_merkle_poseidon_update(leaf: *mut cpb_poseidon_ctx, node: *mut cpb_poseidon_ctx, leaf_nodes: *mut u64, non_leaf_nodes: *mut u64,
                                   n: usize, indexes: *const u64, new_leaves: *const u64, leaf_len: usize, k: usize,
                                   asserted_root: *const u64, applied: *mut c_int) -> c_int;
+    // batched duplex sponges: n sponges over one context sharing one mode, states (n x t elements) in place, *mode read and advanced
+    fn cpb_poseidon_duplex_absorb(ctx: *mut cpb_poseidon_ctx, states: *mut u64, mode: *mut cpb_sponge_mode, input: *const u64, k: usize,
+                                  n: usize) -> c_int;
+    fn cpb_poseidon_duplex_absorb_bytes(ctx: *mut cpb_poseidon_ctx, states: *mut u64, mode: *mut cpb_sponge_mode, input: *const u8,
+                                        len: usize, stride: usize, n: usize) -> c_int;
+    fn cpb_poseidon_duplex_squeeze(ctx: *mut cpb_poseidon_ctx, states: *mut u64, mode: *mut cpb_sponge_mode, out: *mut u64, m: usize,
+                                   canonical: c_int, n: usize) -> c_int;
     // page-lock a `Vec<Fr>`'s storage once so the host-pointer calls copy at full PCIe rate (ABI v3)
     fn cpb_host_register(ptr: *mut core::ffi::c_void, bytes: usize) -> c_int;
     fn cpb_host_unregister(ptr: *mut core::ffi::c_void) -> c_int;
@@ -44,6 +53,15 @@ extern "C" {
     fn cpb_multi_uses_nccl(m: *const cpb_multi) -> c_int;
     fn cpb_merkle_poseidon_build_multi(m: *mut cpb_multi, leaf_ctxs: *const *mut cpb_poseidon_ctx, node_ctxs: *const *mut cpb_poseidon_ctx,
                                        leaves: *const u64, leaf_len: usize, n: usize, leaf_nodes: *mut u64, non_leaf_nodes: *mut u64) -> c_int;
+}
+
+/// `DuplexSpongeMode` (R/sponge/mod.rs): squeezing 0 = Absorbing{next_absorb_index = index}, 1 = Squeezing{index}.
+#[allow(non_camel_case_types)]
+#[repr(C)]
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub struct cpb_sponge_mode {
+    pub squeezing: c_int,
+    pub index: usize,
 }
 
 #[allow(non_camel_case_types)]
@@ -190,6 +208,102 @@ impl<F: GpuField + ark_crypto_primitives::sponge::Absorb> TwoToOneCRHScheme for 
     fn evaluate<T: Borrow<F>>(p: &Self::Parameters, l: T, r: T) -> Result<F, Error> { Self::compress(p, l, r) }
     fn compress<T: Borrow<F>>(p: &Self::Parameters, l: T, r: T) -> Result<F, Error> {
         Ok(Self::compress_batch(p, &[(*l.borrow(), *r.borrow())])?[0])
+    }
+}
+
+/// `PoseidonSponge<F>` (R/sponge/poseidon/mod.rs:47-63) on the GPU: the n = 1 case of the batched duplex.  Every absorb or squeeze
+/// is one library call, which runs the reference's mode bookkeeping (mod.rs:124-186) and every permutation that call needs; the
+/// state stays in host memory between calls.  The trait methods return no `Result`, so a library error panics.
+#[derive(Clone)]
+pub struct GpuPoseidonSponge<F: GpuField> {
+    params: GpuPoseidonParams<F>,
+    state: Vec<u64>,
+    mode: cpb_sponge_mode,
+}
+impl<F: GpuField> GpuPoseidonSponge<F> {
+    fn squeeze_raw(&mut self, m: usize, canonical: bool) -> Vec<u64> {
+        let mut out = vec![0u64; 4 * m];
+        let ptr = if m == 0 { core::ptr::null_mut() } else { out.as_mut_ptr() };
+        check(unsafe { cpb_poseidon_duplex_squeeze(self.params.ctx.0, self.state.as_mut_ptr(), &mut self.mode, ptr, m, canonical as c_int, 1) })
+            .expect("cpb_poseidon_duplex_squeeze");
+        out
+    }
+    /// squeeze_native_field_elements as canonical little-endian integers (4 limbs each): what the byte and bit squeezes cut up.
+    fn squeeze_canonical(&mut self, m: usize) -> Vec<u64> { self.squeeze_raw(m, true) }
+    /// The mode as the reference's `DuplexSpongeMode` would report it.
+    pub fn mode(&self) -> cpb_sponge_mode { self.mode }
+}
+impl<F: GpuField> CryptographicSponge for GpuPoseidonSponge<F> {
+    type Config = GpuPoseidonParams<F>;
+
+    fn new(params: &Self::Config) -> Self {                                                    // mod.rs:220-234
+        let t = params.config.rate + params.config.capacity;
+        Self { params: params.clone(), state: vec![0u64; 4 * t], mode: cpb_sponge_mode { squeezing: 0, index: 0 } }
+    }
+
+    fn absorb(&mut self, input: &impl Absorb) {                                                // mod.rs:236-257
+        let elems = flatten(&input.to_sponge_field_elements_as_vec::<F>());
+        let ptr = if elems.is_empty() { core::ptr::null() } else { elems.as_ptr() };
+        check(unsafe { cpb_poseidon_duplex_absorb(self.params.ctx.0, self.state.as_mut_ptr(), &mut self.mode, ptr, elems.len() / 4, 1) })
+            .expect("cpb_poseidon_duplex_absorb");
+    }
+
+    fn squeeze_bytes(&mut self, num_bytes: usize) -> Vec<u8> {                                 // mod.rs:259-274
+        let usable = ((F::MODULUS_BIT_SIZE - 1) / 8) as usize;
+        let limbs = self.squeeze_canonical((num_bytes + usable - 1) / usable);
+        let mut bytes = Vec::with_capacity(num_bytes + usable);
+        for e in limbs.chunks_exact(4) {
+            let le: Vec<u8> = e.iter().flat_map(|l| l.to_le_bytes()).collect();
+            bytes.extend_from_slice(&le[..usable]);
+        }
+        bytes.truncate(num_bytes);
+        bytes
+    }
+
+    fn squeeze_bits(&mut self, num_bits: usize) -> Vec<bool> {                                 // mod.rs:276-289
+        let usable = (F::MODULUS_BIT_SIZE - 1) as usize;
+        let limbs = self.squeeze_canonical((num_bits + usable - 1) / usable);
+        let mut bits = Vec::with_capacity(num_bits + usable);
+        for e in limbs.chunks_exact(4) {
+            bits.extend((0..usable).map(|i| (e[i / 64] >> (i % 64)) & 1 == 1));
+        }
+        bits.truncate(num_bits);
+        bits
+    }
+
+    // mod.rs:291-307: a native field with every size Full is the native squeeze; everything else is the bit-sampling rule of
+    // R/sponge/mod.rs:57-96 (restated here: the reference's helper is crate-private)
+    fn squeeze_field_elements_with_sizes<F2: PrimeField>(&mut self, sizes: &[FieldElementSize]) -> Vec<F2> {
+        if F::characteristic() == F2::characteristic() && sizes.iter().all(|s| *s == FieldElementSize::Full) {
+            return self.squeeze_native_field_elements(sizes.len()).iter().map(|x| F2::from_le_bytes_mod_order(&x.into_bigint().to_bytes_le())).collect();
+        }
+        if sizes.is_empty() {
+            return Vec::new();
+        }
+        let widths: Vec<usize> = sizes.iter().map(|s| match s {
+            FieldElementSize::Full => (F2::MODULUS_BIT_SIZE - 1) as usize,
+            FieldElementSize::Truncated(b) => {
+                assert!(*b <= F2::MODULUS_BIT_SIZE as usize, "num_bits is greater than the capacity of the field.");
+                *b
+            },
+        }).collect();
+        let bits = self.squeeze_bits(widths.iter().sum());
+        let mut pos = 0;
+        widths.iter().map(|&w| {
+            let bytes: Vec<u8> = bits[pos..pos + w].chunks(8)
+                .map(|c| c.iter().enumerate().fold(0u8, |acc, (i, &b)| acc | ((b as u8) << i))).collect();
+            pos += w;
+            F2::from_le_bytes_mod_order(&bytes)
+        }).collect()
+    }
+
+    fn squeeze_field_elements<F2: PrimeField>(&mut self, num_elements: usize) -> Vec<F2> {      // mod.rs:309-320
+        self.squeeze_field_elements_with_sizes::<F2>(vec![FieldElementSize::Full; num_elements].as_slice())
+    }
+}
+impl<F: GpuField> FieldBasedCryptographicSponge<F> for GpuPoseidonSponge<F> {
+    fn squeeze_native_field_elements(&mut self, num_elements: usize) -> Vec<F> {              // mod.rs:323-345
+        unflatten(&self.squeeze_raw(num_elements, false))
     }
 }
 
