@@ -69,6 +69,12 @@ SIGNATURES = {
     "cpb_poseidon_duplex_absorb_bytes_dev": (C.c_int, [vp, vp, modep, vp, C.c_size_t, C.c_size_t, C.c_size_t, vp]),
     "cpb_poseidon_duplex_squeeze": (C.c_int, [vp, u64p, modep, u64p, C.c_size_t, C.c_int, C.c_size_t]),
     "cpb_poseidon_duplex_squeeze_dev": (C.c_int, [vp, vp, modep, vp, C.c_size_t, C.c_int, C.c_size_t, vp]),
+    "cpb_poseidon_duplex_absorb_ragged": (C.c_int, [vp, u64p, modep, u64p, u64p, C.c_size_t]),
+    "cpb_poseidon_duplex_absorb_ragged_dev": (C.c_int, [vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    "cpb_poseidon_duplex_absorb_bytes_ragged": (C.c_int, [vp, u64p, modep, u8p, u64p, C.c_size_t]),
+    "cpb_poseidon_duplex_absorb_bytes_ragged_dev": (C.c_int, [vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    "cpb_poseidon_duplex_squeeze_ragged": (C.c_int, [vp, u64p, modep, u64p, u64p, C.c_int, C.c_size_t]),
+    "cpb_poseidon_duplex_squeeze_ragged_dev": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, C.c_size_t, vp]),
     "cpb_merkle_poseidon_build": (C.c_int, [vp, vp, u64p, C.c_size_t, C.c_size_t, u64p, u64p]),
     "cpb_merkle_poseidon_build_dev": (C.c_int, [vp, vp, vp, C.c_size_t, C.c_size_t, vp, vp, vp]),
     "cpb_merkle_poseidon_from_digests": (C.c_int, [vp, u64p, C.c_size_t, u64p]),

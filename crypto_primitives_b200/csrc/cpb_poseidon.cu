@@ -10,6 +10,7 @@
 //   k_field_convert     canonical <-> Montgomery.
 // Round constants / MDS / sparse rows are staged into shared memory with one TMA bulk copy per
 // CTA; inputs are read with 128-bit loads; state lives in registers.
+#include <cstddef>
 #include <cstdlib>
 #include <vector>
 
@@ -384,7 +385,8 @@ size_t count_launches(const cpb_poseidon_ctx* node, size_t n) {
 bool pow2_gt1(size_t n) { return n > 1 && (n & (n - 1)) == 0; }
 
 // ------------------------------------------------------------------------------ ragged batches
-// Counting sort of the items by absorb-permutation count (ragged_key, poseidon.cuh) into order[n]: a histogram, an exclusive
+// Counting sort of the items by a key (the CRH: absorb-permutation count, ragged_key in poseidon.cuh; the duplex: permutations of
+// the call, duplex_ragged_key in poseidon_duplex.cuh) into order[n]: a histogram, an exclusive
 // scan, a scatter.  Each CTA of the histogram and scatter kernels owns kSortBlock * kSortItems consecutive items; the scatter
 // reserves one slice per bucket with one global atomic, so items of a bucket stay in CTA-sized runs of nearby inputs.
 constexpr int kSortBlock = 256, kSortItems = 8;
@@ -406,7 +408,21 @@ __device__ __forceinline__ unsigned warp_aggregated_inc(unsigned* counter, int k
     return base + __popc(peers & ((1u << lane) - 1u));
 }
 
-__global__ void __launch_bounds__(kSortBlock) k_ragged_hist(const u64* __restrict__ offsets, long n, int rate, unsigned* __restrict__ hist) {
+// Key sources of the counting sort: item i's bucket, 0 .. kRaggedBuckets-1.
+struct CrhKey {                         // absorb permutations of a ragged hash input
+    const u64* offsets;
+    long n;
+    int rate;
+    __device__ int operator()(long i) const { return ragged_key(ragged_span(offsets, i, n).len, rate); }
+};
+struct DuplexKey {                      // permutations of a sponge's part of a ragged duplex call
+    DuplexRagged R;
+    long rate;
+    __device__ int operator()(long i) const { return duplex_ragged_key(R, i, rate); }
+};
+
+template <class Key>
+__global__ void __launch_bounds__(kSortBlock) k_ragged_hist(Key key, long n, unsigned* __restrict__ hist) {
     __shared__ unsigned h[kRaggedBuckets];
     for (int b = threadIdx.x; b < kRaggedBuckets; b += kSortBlock) h[b] = 0;
     __syncthreads();
@@ -414,7 +430,7 @@ __global__ void __launch_bounds__(kSortBlock) k_ragged_hist(const u64* __restric
 #pragma unroll
     for (int k = 0; k < kSortItems; k++) {
         const long i = first + (long)k * kSortBlock;
-        if (i < n) warp_aggregated_inc(h, ragged_key(ragged_span(offsets, i, n).len, rate));
+        if (i < n) warp_aggregated_inc(h, key(i));
     }
     __syncthreads();
     for (int b = threadIdx.x; b < kRaggedBuckets; b += kSortBlock)
@@ -428,22 +444,22 @@ __global__ void k_ragged_scan(RaggedHeader* H, int single) {
     ragged_ranges(H->starts, single != 0, H->range);
 }
 
-__global__ void __launch_bounds__(kSortBlock) k_ragged_scatter(const u64* __restrict__ offsets, long n, int rate, unsigned* __restrict__ cursor,
-                                                               unsigned* __restrict__ order) {
+template <class Key>
+__global__ void __launch_bounds__(kSortBlock) k_ragged_scatter(Key key, long n, unsigned* __restrict__ cursor, unsigned* __restrict__ order) {
     __shared__ unsigned h[kRaggedBuckets], base[kRaggedBuckets];
     for (int b = threadIdx.x; b < kRaggedBuckets; b += kSortBlock) h[b] = 0;
     __syncthreads();
     const long first = (long)blockIdx.x * (kSortBlock * kSortItems) + threadIdx.x;
-    int key[kSortItems];
+    int kb[kSortItems];
     unsigned slot[kSortItems];
 #pragma unroll
     for (int k = 0; k < kSortItems; k++) {
         const long i = first + (long)k * kSortBlock;
-        key[k] = 0;
+        kb[k] = 0;
         slot[k] = 0;
         if (i < n) {
-            key[k] = ragged_key(ragged_span(offsets, i, n).len, rate);
-            slot[k] = warp_aggregated_inc(h, key[k]);
+            kb[k] = key(i);
+            slot[k] = warp_aggregated_inc(h, kb[k]);
         }
     }
     __syncthreads();
@@ -452,12 +468,13 @@ __global__ void __launch_bounds__(kSortBlock) k_ragged_scatter(const u64* __rest
 #pragma unroll
     for (int k = 0; k < kSortItems; k++) {
         const long i = first + (long)k * kSortBlock;
-        if (i < n) order[base[key[k]] + slot[k]] = (unsigned)i;
+        if (i < n) order[base[kb[k]] + slot[k]] = (unsigned)i;
     }
 }
 
 // CPB_RAGGED_ORDER=0 (read once) hashes ragged batches in input order with one sponge launch and no ordering step.  It exists
-// only to measure what the ordering buys (tools/perf_ragged.py); results are the same either way.
+// only to measure what the ordering buys (tools/perf_ragged.py; for ragged duplex calls tools/perf_duplex_ragged.py); results are
+// the same either way.
 bool ragged_order_enabled() {
     static int v = -1;
     if (v < 0) {
@@ -482,14 +499,15 @@ static cpb_status hash_ragged(cpb_poseidon_ctx* c, const u32* values, u64 vbase,
     return fail(CPB_UNSUPPORTED, "state width t=%d is not built (this library: t = 2..9)", c->dev.t);
 }
 
-static cpb_status order_ragged(const u64* offsets, size_t n, int rate, bool single, RaggedHeader* H, unsigned* order, cudaStream_t st) {
+template <class Key>
+static cpb_status order_ragged(Key key, size_t n, bool single, RaggedHeader* H, unsigned* order, cudaStream_t st) {
     const unsigned grid = (unsigned)((n + kSortBlock * kSortItems - 1) / (kSortBlock * kSortItems));
     CPB_CUDA(cudaMemsetAsync(H->hist, 0, sizeof(H->hist), st));
-    k_ragged_hist<<<grid, kSortBlock, 0, st>>>(offsets, (long)n, rate, H->hist);
+    k_ragged_hist<<<grid, kSortBlock, 0, st>>>(key, (long)n, H->hist);
     CPB_CUDA(cudaGetLastError());
     k_ragged_scan<<<1, 32, 0, st>>>(H, single ? 1 : 0);
     CPB_CUDA(cudaGetLastError());
-    k_ragged_scatter<<<grid, kSortBlock, 0, st>>>(offsets, (long)n, rate, H->cursor, order);
+    k_ragged_scatter<<<grid, kSortBlock, 0, st>>>(key, (long)n, H->cursor, order);
     CPB_CUDA(cudaGetLastError());
     return CPB_OK;
 }
@@ -507,7 +525,7 @@ cpb_status launch_crh_ragged(cpb_poseidon_ctx* c, const u32* values, u64 vbase, 
     CPB_CUDA(cudaMallocAsync((void**)&tmp, hdr + n * sizeof(unsigned), st));
     RaggedHeader* H = reinterpret_cast<RaggedHeader*>(tmp);
     unsigned* order = reinterpret_cast<unsigned*>(tmp + hdr);
-    cpb_status rc = order_ragged(offsets, n, c->dev.rate, single, H, order, st);
+    cpb_status rc = order_ragged(CrhKey{offsets, (long)n, c->dev.rate}, n, single, H, order, st);
     if (rc == CPB_OK) rc = hash_ragged(c, values, vbase, offsets, order, H->range, out, n_out, n, single, st);
     cudaFreeAsync(tmp, st);
     return rc;
@@ -533,18 +551,19 @@ cpb_status check_offsets(const uint64_t* offsets, size_t n) {
 }
 
 // Copies a ragged host batch into `buf`: the n + 1 offsets at d_off, then values[offsets[0] .. offsets[n]) at d_val (so the
-// device values start at index vbase = offsets[0]).  `front` bytes at the start of buf are left to the caller.
-cpb_status stage_ragged(Scratch& buf, size_t front, const uint64_t* values, const uint64_t* offsets, size_t n, cudaStream_t st,
-                        u64*& d_off, u32*& d_val) {
+// device values start at index vbase = offsets[0]).  `front` bytes at the start of buf are left to the caller.  `unit`: bytes per
+// offset step (32 for field elements, 1 for byte strings, 0 to copy offsets only).
+cpb_status stage_ragged(Scratch& buf, size_t front, const void* values, const uint64_t* offsets, size_t n, cudaStream_t st,
+                        u64*& d_off, u32*& d_val, size_t unit = 32) {
     auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t b_off = (n + 1) * 8, b_val = (size_t)(offsets[n] - offsets[0]) * 32;
+    const size_t b_off = (n + 1) * 8, b_val = (size_t)(offsets[n] - offsets[0]) * unit;
     const size_t o_off = up(front), o_val = o_off + up(b_off);
     CPB_TRY(buf.reserve(o_val + (b_val ? b_val : 32)));
     char* d = (char*)buf.ptr;
     d_off = (u64*)(d + o_off);
     d_val = (u32*)(d + o_val);
     CPB_CUDA(cudaMemcpyAsync(d_off, offsets, b_off, cudaMemcpyHostToDevice, st));
-    if (b_val) CPB_CUDA(cudaMemcpyAsync(d_val, values + 4 * offsets[0], b_val, cudaMemcpyHostToDevice, st));
+    if (b_val) CPB_CUDA(cudaMemcpyAsync(d_val, (const char*)values + unit * offsets[0], b_val, cudaMemcpyHostToDevice, st));
     return CPB_OK;
 }
 
@@ -1236,6 +1255,81 @@ cpb_status duplex_squeeze(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode
     return duplex_call(c, states, mode, op, n, 0, n * m * 32, host, (cudaStream_t)stream);
 }
 
+static_assert(sizeof(cpb_sponge_mode) == 16 && offsetof(cpb_sponge_mode, squeezing) == 0 && offsetof(cpb_sponge_mode, index) == 8,
+              "the ragged duplex kernels read and write cpb_sponge_mode as two 64-bit words");
+
+cpb_status launch_duplex_ragged(cpb_poseidon_ctx* c, u32* states, const DuplexRagged& R, const unsigned* order, cudaStream_t st) {
+    CPB_FOR_FIELD(launch_duplex_ragged_ft, c, states, R, order, st)
+    return fail(CPB_UNSUPPORTED, "state width t=%d is not built (this library: t = 2..9)", c->dev.t);
+}
+
+// One ragged call on device arrays: the sponges sorted by their permutation count (DuplexKey), then one launch over the order.
+// The ordering scratch comes from the stream-ordered pool, so nothing here synchronises the host.
+cpb_status duplex_ragged_dev(cpb_poseidon_ctx* c, u32* states, const DuplexRagged& R, cudaStream_t st) {
+    if (!ragged_order_enabled()) return launch_duplex_ragged(c, states, R, nullptr, st);
+    const size_t hdr = (sizeof(RaggedHeader) + 255) & ~(size_t)255;
+    char* tmp = nullptr;
+    CPB_CUDA(cudaMallocAsync((void**)&tmp, hdr + (size_t)R.n * sizeof(unsigned), st));
+    RaggedHeader* H = reinterpret_cast<RaggedHeader*>(tmp);
+    unsigned* order = reinterpret_cast<unsigned*>(tmp + hdr);
+    cpb_status rc = order_ragged(DuplexKey{R, c->dev.rate}, (size_t)R.n, false, H, order, st);
+    if (rc == CPB_OK) rc = launch_duplex_ragged(c, states, R, order, st);
+    cudaFreeAsync(tmp, st);
+    return rc;
+}
+
+// A ragged duplex call (kind: DuplexKind; data: the elements, the bytes or the output buffer).  The checks come in the header's
+// order; the host form's checks of its host arrays come before the context, except the mode index against the rate.
+cpb_status duplex_ragged(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* modes, int kind, void* data, const uint64_t* offsets,
+                         size_t n, bool host, void* stream) {
+    if (n >= ((size_t)1 << 32)) return fail(CPB_BAD_LENGTH, "a ragged batch holds fewer than 2^32 sponges (got %zu)", n);
+    if (n == 0) return CPB_OK;
+    if (!states || !modes || !offsets) return fail(CPB_NULL_POINTER, "null buffer");
+    const size_t unit = kind == kAbsorbBytes ? 1 : 32;
+    if (host) {
+        CPB_TRY(check_offsets(offsets, n));
+        if (!fits(offsets[n] - offsets[0], unit)) return fail(CPB_BAD_LENGTH, "spans too large (%llu)", (unsigned long long)(offsets[n] - offsets[0]));
+        if (!data && offsets[n] != offsets[0]) return fail(CPB_NULL_POINTER, "null data buffer");
+        for (size_t i = 0; i < n; i++)
+            if (modes[i].squeezing != 0 && modes[i].squeezing != 1)
+                return fail(CPB_BAD_PARAMS, "modes[%zu].squeezing must be 0 or 1 (got %d)", i, modes[i].squeezing);
+    }
+    CPB_TRY(check_ctx(c));
+    const long rate = c->dev.rate;
+    if (host)
+        for (size_t i = 0; i < n; i++)
+            if (!duplex_mode_valid(modes[i].squeezing, modes[i].index, rate))
+                return fail(CPB_BAD_PARAMS, "modes[%zu].index %zu exceeds the rate %ld", i, modes[i].index, rate);
+    DuplexRagged R{kind, (u64*)modes, offsets, 0, (const u32*)data, (const unsigned char*)data, (u32*)data, (long)n};
+    DeviceGuard g(c->device);
+    if (!host) return duplex_ragged_dev(c, (u32*)states, R, (cudaStream_t)stream);
+
+    // host form: states in s_aux; the modes, the offsets and the data span in s_in; the output span in s_out
+    std::lock_guard<std::mutex> lk(c->mu);
+    cudaStream_t st = c->stream;
+    const bool squeeze = kind >= kSqueeze;
+    const size_t s_b = n * (size_t)c->dev.t * 32, m_b = n * sizeof(cpb_sponge_mode), span = (size_t)(offsets[n] - offsets[0]);
+    CPB_TRY(c->s_aux.reserve(s_b));
+    u64* d_off = nullptr;
+    u32* d_val = nullptr;
+    CPB_TRY(stage_ragged(c->s_in, m_b, data, offsets, n, st, d_off, d_val, squeeze ? 0 : unit));
+    if (squeeze) CPB_TRY(c->s_out.reserve(span ? span * 32 : 32));
+    CPB_CUDA(cudaMemcpyAsync(c->s_aux.ptr, states, s_b, cudaMemcpyHostToDevice, st));
+    CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, modes, m_b, cudaMemcpyHostToDevice, st));
+    R.modes = (u64*)c->s_in.ptr;
+    R.offsets = d_off;
+    R.vbase = offsets[0];
+    R.in = d_val;
+    R.bytes = (const unsigned char*)d_val;
+    R.out = squeeze ? (u32*)c->s_out.ptr : nullptr;
+    CPB_TRY(duplex_ragged_dev(c, (u32*)c->s_aux.ptr, R, st));
+    CPB_CUDA(cudaMemcpyAsync(states, c->s_aux.ptr, s_b, cudaMemcpyDeviceToHost, st));
+    CPB_CUDA(cudaMemcpyAsync(modes, c->s_in.ptr, m_b, cudaMemcpyDeviceToHost, st));
+    if (squeeze && span) CPB_CUDA(cudaMemcpyAsync((uint64_t*)data + 4 * offsets[0], c->s_out.ptr, span * 32, cudaMemcpyDeviceToHost, st));
+    CPB_CUDA(cudaStreamSynchronize(st));
+    return CPB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1262,6 +1356,35 @@ cpb_status cpb_poseidon_duplex_squeeze(cpb_poseidon_ctx* c, uint64_t* states, cp
 cpb_status cpb_poseidon_duplex_squeeze_dev(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, uint64_t* out, size_t m,
                                            int canonical, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status { return duplex_squeeze(c, states, mode, out, m, canonical, n, false, stream); });
+}
+
+cpb_status cpb_poseidon_duplex_absorb_ragged(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* modes, const uint64_t* values,
+                                             const uint64_t* offsets, size_t n) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_ragged(c, states, modes, kAbsorb, (void*)values, offsets, n, true, nullptr); });
+}
+cpb_status cpb_poseidon_duplex_absorb_ragged_dev(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* modes, const uint64_t* values,
+                                                 const uint64_t* offsets, size_t n, void* stream) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_ragged(c, states, modes, kAbsorb, (void*)values, offsets, n, false, stream); });
+}
+cpb_status cpb_poseidon_duplex_absorb_bytes_ragged(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* modes, const uint8_t* bytes,
+                                                   const uint64_t* offsets, size_t n) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_ragged(c, states, modes, kAbsorbBytes, (void*)bytes, offsets, n, true, nullptr); });
+}
+cpb_status cpb_poseidon_duplex_absorb_bytes_ragged_dev(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* modes, const uint8_t* bytes,
+                                                       const uint64_t* offsets, size_t n, void* stream) {
+    return cpb::guarded([&]() -> cpb_status { return duplex_ragged(c, states, modes, kAbsorbBytes, (void*)bytes, offsets, n, false, stream); });
+}
+cpb_status cpb_poseidon_duplex_squeeze_ragged(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* modes, uint64_t* out,
+                                              const uint64_t* offsets, int canonical, size_t n) {
+    return cpb::guarded([&]() -> cpb_status {
+        return duplex_ragged(c, states, modes, canonical ? kSqueezeCanonical : kSqueeze, out, offsets, n, true, nullptr);
+    });
+}
+cpb_status cpb_poseidon_duplex_squeeze_ragged_dev(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* modes, uint64_t* out,
+                                                  const uint64_t* offsets, int canonical, size_t n, void* stream) {
+    return cpb::guarded([&]() -> cpb_status {
+        return duplex_ragged(c, states, modes, canonical ? kSqueezeCanonical : kSqueeze, out, offsets, n, false, stream);
+    });
 }
 
 }  // extern "C"

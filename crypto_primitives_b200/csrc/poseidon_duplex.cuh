@@ -1,7 +1,8 @@
 // poseidon_duplex.cuh -- batched duplex sponges: n PoseidonSponge<F> over one PoseidonConfig, states in device memory, one
 // DuplexSpongeMode shared by the batch (R/sponge/poseidon/mod.rs:47-63).  Every call applies the same absorb or squeeze to all n
 // sponges with per-sponge data, so the mode bookkeeping is uniform: the host runs duplex_plan to advance the mode and to form the
-// launch arguments, and the kernel runs the same plan (carried in DuplexOp) to drive its loop.
+// launch arguments, and the kernel runs the same plan (carried in DuplexOp) to drive its loop.  A ragged call gives every sponge its
+// own mode and its own span: duplex_step runs the same plan per item on the device, and pos_duplex_ragged runs pos_duplex on it.
 //
 // Everything here is CPB_HD so that tests/host can run the plan and the byte encoding on the CPU against the oracle.
 #pragma once
@@ -141,6 +142,79 @@ CPB_HD void pos_duplex(u32* state, const DuplexOp& op, long i, const PoseidonDev
     }
 #pragma unroll
     for (int j = 0; j < T; j++) st_elem(state + 8 * j, s[j]);
+}
+
+// ---- ragged calls: every sponge has its own mode and its own span (poseidon.cuh: ragged_span), so the mode bookkeeping is per item
+// and runs where the item runs.  Modes are n cpb_sponge_mode in memory, two 64-bit words each: squeezing in the low 4 bytes of word
+// 0 (the upper 4 are padding and are not read) and index in word 1.  A stored mode writes both words whole, the padding zeroed.
+struct DuplexRagged {
+    int kind;                    // DuplexKind
+    u64* modes;                  // n x 2 words, read and updated
+    const u64* offsets;          // n + 1; sponge i's span is [offsets[i], offsets[i+1]) in elements (kAbsorbBytes: bytes)
+    u64 vbase;                   // the offset that the data pointers' first element stands for
+    const u32* in;               // kAbsorb
+    const unsigned char* bytes;  // kAbsorbBytes
+    u32* out;                    // kSqueeze, kSqueezeCanonical
+    long n;
+};
+
+// What one sponge's part of a ragged call does: `op` is rebased to the item (pos_duplex with i = 0 reads or writes its span), `mode`
+// the mode after it, `perms` its permutations (permute_first + boundaries; 0 for a no-op).  A sponge whose stored mode is not one the
+// reference can be in (duplex_mode_valid) is not valid: it is left untouched and its squeeze span is zeroed.
+struct DuplexStep {
+    bool valid, noop;
+    DuplexOp op;
+    DuplexMode mode;
+    long perms;
+};
+
+CPB_HD DuplexStep duplex_step(int kind, int squeezing, unsigned long long index, RaggedSpan sp, const DuplexRagged& R, long rate) {
+    DuplexStep s{false, true, DuplexOp{kind, 0, 0, 0, 0, nullptr, nullptr, 0, 0, nullptr}, DuplexMode{squeezing, 0}, 0};
+    const long off = (long)(sp.lo - R.vbase);
+    s.op.count = kind == kAbsorbBytes ? duplex_byte_elems(sp.len) : sp.len;
+    if (kind == kAbsorb) s.op.in = R.in + 8 * off;
+    else if (kind == kAbsorbBytes) {
+        s.op.bytes = R.bytes + off;
+        s.op.len = sp.len;
+    } else s.op.out = R.out + 8 * off;
+    if (!duplex_mode_valid(squeezing, index, rate)) return s;
+    const DuplexPlan p = duplex_plan(kind >= kSqueeze, DuplexMode{squeezing, (long)index}, rate, s.op.count);
+    s.valid = true;
+    s.noop = p.noop;
+    s.op.first = p.permute_first ? 1 : 0;
+    s.op.start = p.start;
+    s.op.boundaries = p.boundaries;
+    s.mode = p.mode;
+    s.perms = p.noop ? 0 : s.op.first + p.boundaries;
+    return s;
+}
+
+// Sponge i's step as read from memory: its stored mode and its clamped span.
+CPB_HD DuplexStep duplex_ragged_step(const DuplexRagged& R, long i, long rate) {
+    return duplex_step(R.kind, (int)(u32)R.modes[2 * i], R.modes[2 * i + 1], ragged_span(R.offsets, i, R.n), R, rate);
+}
+// The ordering key of sponge i: its permutation count, clamped at kRaggedBuckets - 1.
+CPB_HD int duplex_ragged_key(const DuplexRagged& R, long i, long rate) {
+    const long p = duplex_ragged_step(R, i, rate).perms;
+    return (int)(p < kRaggedBuckets - 1 ? p : kRaggedBuckets - 1);
+}
+
+// Sponge i's whole part of a ragged call (one thread of k_poseidon_duplex_ragged): the unchanged per-sponge body on the rebased op,
+// then the new mode.
+template <class F, int T>
+CPB_HD void pos_duplex_ragged(u32* states, const DuplexRagged& R, long i, const PoseidonDev& P, const u32* cs, const u32* pm) {
+    const DuplexStep s = duplex_ragged_step(R, i, P.rate);
+    if (!s.valid) {
+        if (R.kind >= kSqueeze) {
+            u32 z[8];
+            fp_zero(z);
+            for (long e = 0; e < s.op.count; e++) st_elem(s.op.out + 8 * e, z);
+        }
+        return;
+    }
+    if (!s.noop) pos_duplex<F, T>(states + 8 * T * i, s.op, 0, P, cs, pm);
+    R.modes[2 * i] = (u64)s.mode.squeezing;
+    R.modes[2 * i + 1] = (u64)s.mode.index;
 }
 
 }  // namespace cpb

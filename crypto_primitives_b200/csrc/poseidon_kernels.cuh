@@ -402,6 +402,33 @@ cpb_status launch_duplex_ft(cpb_poseidon_ctx* c, u32* states, const DuplexOp& op
     return CPB_OK;
 }
 
+// Ragged duplex calls (poseidon_duplex.cuh: pos_duplex_ragged): one sponge per thread, slot j is sponge order[j] (order == nullptr:
+// input order).  No grid-stride loop, as in k_poseidon_crh_ragged: R.n < 2^32 (checked by the caller).
+template <class F, int T>
+__global__ void __launch_bounds__(kBlock, pos_min_blocks(T))
+k_poseidon_duplex_ragged(PoseidonDev P, const u32* __restrict__ consts, u32* __restrict__ states, DuplexRagged R,
+                         const unsigned* __restrict__ order) {
+    extern __shared__ __align__(16) u32 cs[];
+    __shared__ __align__(8) unsigned long long mbar;
+    tma_stage_to_smem(cs, consts, (unsigned)P.n_elems * 32u, &mbar);
+    const long j = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= R.n) return;
+    const u32* ct = cs + (int)threadIdx.x * P.zero;
+    u32 pm[8];
+    ld_elem(pm, ct + 8 * P.off_mod);
+    pos_duplex_ragged<F, T>(states, R, order ? (long)order[j] : j, P, ct, pm);
+}
+
+template <class F, int T>
+cpb_status launch_duplex_ragged_ft(cpb_poseidon_ctx* c, u32* states, const DuplexRagged& R, const unsigned* order, cudaStream_t st) {
+    size_t smem = (size_t)c->dev.n_elems * 32;
+    int grid = 1;
+    CPB_TRY(grid_ragged(k_poseidon_duplex_ragged<F, T>, smem, (size_t)R.n, grid));
+    k_poseidon_duplex_ragged<F, T><<<grid, kBlock, smem, st>>>(c->dev, c->d_consts, states, R, order);
+    CPB_CUDA(cudaGetLastError());
+    return CPB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Tree-top kernel: ALL the small levels of a Merkle (sub)tree in one launch, four warps per 32 hashes
 // (poseidon_team.cuh), and -- on a multi-GPU build -- the exchange of the subtree roots over NVLink peer memory and
@@ -652,8 +679,13 @@ cpb_status merkle_build_streams(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, 
     extern template cpb_status launch_verify_digests_ft<F, T>(cpb_poseidon_ctx*, const u32*, const u32*, const u32*, const u32*, \
                                                               int, const unsigned long long*, unsigned char*, size_t, cudaStream_t);
 // the duplex kernels (poseidon_duplex_<field>.cu), likewise in units of their own
-#define CPB_POS_INSTANTIATE_DUPLEX(F, T) template cpb_status launch_duplex_ft<F, T>(cpb_poseidon_ctx*, u32*, const DuplexOp&, size_t, cudaStream_t);
-#define CPB_POS_EXTERN_DUPLEX(F, T) extern template cpb_status launch_duplex_ft<F, T>(cpb_poseidon_ctx*, u32*, const DuplexOp&, size_t, cudaStream_t);
+#define CPB_POS_INSTANTIATE_DUPLEX(F, T)                                                                                 \
+    template cpb_status launch_duplex_ft<F, T>(cpb_poseidon_ctx*, u32*, const DuplexOp&, size_t, cudaStream_t);          \
+    template cpb_status launch_duplex_ragged_ft<F, T>(cpb_poseidon_ctx*, u32*, const DuplexRagged&, const unsigned*, cudaStream_t);
+#define CPB_POS_EXTERN_DUPLEX(F, T)                                                                                      \
+    extern template cpb_status launch_duplex_ft<F, T>(cpb_poseidon_ctx*, u32*, const DuplexOp&, size_t, cudaStream_t);   \
+    extern template cpb_status launch_duplex_ragged_ft<F, T>(cpb_poseidon_ctx*, u32*, const DuplexRagged&, const unsigned*,  \
+                                                             cudaStream_t);
 #define CPB_POS_INSTANTIATE_TEAM(F) template cpb_status launch_tree_top_f<F>(cpb_poseidon_ctx*, TopJob, cudaStream_t);
 #define CPB_POS_EXTERN_TEAM(F) extern template cpb_status launch_tree_top_f<F>(cpb_poseidon_ctx*, TopJob, cudaStream_t);
 #define CPB_POS_EXTERN(F, T)                                                                                             \

@@ -319,7 +319,8 @@ class PoseidonSpongeBatch:
                 raise ValueError(f"expected {self.n} absorbables, one per sponge (got {len(items)})")
             enc = [to_sponge_field_elements(v, self.parameters.field) for v in items]
             if len({a.shape[0] for a in enc}) > 1:
-                raise ValueError("the items encode to different numbers of field elements; a batch absorbs one length")
+                raise ValueError("the items encode to different numbers of field elements; a batch absorbs one length "
+                                 "(RaggedPoseidonSpongeBatch absorbs each at its own)")
             e = _as_i64(np.stack(enc) if enc else np.zeros((0, 0, 4), dtype=np.uint64), self.device)
         e = e.reshape(self.n, -1, 4).contiguous()
         k = e.shape[1]
@@ -414,6 +415,163 @@ class PoseidonSpongeBatch:
         N.check(N.lib.cpb_field_to_montgomery_dev(field.id, self.device.index, limbs.data_ptr(), limbs.data_ptr(), self.n * S,
                                                   self._stream()))
         return limbs
+
+
+class RaggedPoseidonSpongeBatch:
+    """n independent PoseidonSponge over one PoseidonConfig, each with its own DuplexSpongeMode, so that every call can absorb or
+    squeeze a different number of elements per sponge (transcripts whose messages, labels or challenge counts differ).  States are a
+    torch CUDA int64 tensor (n, t, 4) of Montgomery limbs, modes an int64 tensor (n, 2) of [squeezing, index] rows (the
+    cpb_sponge_mode layout), both on `device`.  Every call is one _dev call of the C-ABI (cpb_poseidon_duplex_*_ragged) on the current
+    torch stream: the device sorts the sponges by their permutation count and runs every permutation of the call in one launch.
+    Ragged data is (values, offsets): sponge i's part is values[offsets[i] .. offsets[i+1])."""
+
+    def __init__(self, parameters: PoseidonConfig, n: int, device=None):
+        import torch
+        self.parameters = parameters
+        self.n = int(n)
+        self.device = _cuda_device(device)
+        t = parameters.rate + parameters.capacity
+        self.states = torch.zeros((self.n, t, 4), dtype=torch.int64, device=self.device)
+        self.modes = torch.zeros((self.n, 2), dtype=torch.int64, device=self.device)
+
+    # -- state
+    @classmethod
+    def from_batch(cls, batch: PoseidonSpongeBatch) -> "RaggedPoseidonSpongeBatch":
+        """A copy of a PoseidonSpongeBatch: its states, and its one mode in every row."""
+        b = cls(batch.parameters, batch.n, batch.device)
+        b.states = batch.states.clone()
+        b.modes[:, 0] = int(batch._mode.squeezing)
+        b.modes[:, 1] = int(batch._mode.index)
+        return b
+
+    @classmethod
+    def from_states(cls, states, modes, parameters: PoseidonConfig, device=None) -> "RaggedPoseidonSpongeBatch":
+        """states (n, t, 4) Montgomery limbs and modes (n, 2) [squeezing, index] rows, torch or numpy."""
+        dev = _cuda_device(device)
+        st = _as_i64(states, dev)
+        md = _as_i64(modes, dev)
+        t = parameters.rate + parameters.capacity
+        if st.ndim != 3 or tuple(st.shape[1:]) != (t, 4):
+            raise ValueError(f"states must be (n, {t}, 4)")
+        if tuple(md.shape) != (st.shape[0], 2):
+            raise ValueError(f"modes must be (n={st.shape[0]}, 2)")
+        b = cls(parameters, st.shape[0], st.device)
+        b.states = st.clone()
+        b.modes = md.clone()
+        return b
+
+    def into_states(self):
+        return self.states, self.modes
+
+    def clone(self) -> "RaggedPoseidonSpongeBatch":
+        c = RaggedPoseidonSpongeBatch.__new__(RaggedPoseidonSpongeBatch)
+        c.parameters, c.n, c.device = self.parameters, self.n, self.device
+        c.states, c.modes = self.states.clone(), self.modes.clone()
+        return c
+
+    def sponge(self, i: int) -> PoseidonSponge:
+        """Item i as an independent PoseidonSponge (host state) in its own mode."""
+        st = self.states[i].cpu().numpy().view(np.uint64)
+        sq, idx = (int(v) for v in self.modes[i].cpu())
+        return PoseidonSponge.from_state((st, _py_mode(N.SpongeMode(sq & 0xFFFFFFFF, idx))), self.parameters, self.device.index)
+
+    # -- internals
+    def _call(self, fn, data, offsets, *args):
+        import torch
+        N.check(fn(self.parameters.context(self.device.index), self.states.data_ptr(), self.modes.data_ptr(),
+                   data.data_ptr() if data.numel() else None, offsets.data_ptr(), *args, self.n,
+                   torch.cuda.current_stream(self.device).cuda_stream))
+
+    def _offsets(self, offsets):
+        import torch
+        if isinstance(offsets, np.ndarray):
+            offsets = torch.from_numpy(np.ascontiguousarray(offsets, dtype=np.uint64).view(np.int64))
+        off = torch.as_tensor(offsets, dtype=torch.int64).to(self.device).reshape(-1).contiguous()
+        if off.shape[0] != self.n + 1:
+            raise ValueError(f"offsets needs n + 1 = {self.n + 1} entries (got {off.shape[0]})")
+        return off
+
+    def _pack(self, parts, dtype):
+        """Per-item parts -> (values, offsets) on the device."""
+        import torch
+        if len(parts) != self.n:
+            raise ValueError(f"expected {self.n} items, one per sponge (got {len(parts)})")
+        off = np.zeros(self.n + 1, dtype=np.int64)
+        np.cumsum([len(x) for x in parts], out=off[1:])
+        vals = np.concatenate(parts) if parts else np.zeros((0,), dtype=dtype)
+        return torch.from_numpy(np.ascontiguousarray(vals).view(np.int64 if dtype == np.uint64 else np.uint8)).to(self.device), \
+            torch.from_numpy(off).to(self.device)
+
+    # -- absorb
+    def absorb(self, x):
+        """x: a (values (S, 4), offsets (n + 1)) tuple of Montgomery limbs, torch or numpy; or a list of n items, one per sponge, each a
+        (L_i, 4) limb array or any absorbable of sponge/absorb.py, encoded at its own length."""
+        import torch
+        if isinstance(x, tuple):
+            values, offsets = x
+            v = _as_i64(values, self.device).reshape(-1, 4)
+            off = self._offsets(offsets)
+        else:
+            from .absorb import to_sponge_field_elements
+            parts = []
+            for item in x:
+                if isinstance(item, torch.Tensor):
+                    item = item.cpu().numpy()
+                if isinstance(item, np.ndarray) and item.dtype in (np.uint64, np.int64) and item.ndim == 2 and item.shape[1] == 4:
+                    parts.append(np.ascontiguousarray(item).view(np.uint64))
+                else:
+                    parts.append(to_sponge_field_elements(item, self.parameters.field))
+            v, off = self._pack([p.reshape(-1, 4) for p in parts], np.uint64)
+            v = v.reshape(-1, 4)
+        self._call(N.lib.cpb_poseidon_duplex_absorb_ragged_dev, v, off)
+
+    def absorb_bytes(self, x):
+        """x: a list of n `bytes`, one [u8] value per sponge, or a (uint8 values, offsets (n + 1)) tuple."""
+        import torch
+        if isinstance(x, tuple):
+            values, offsets = x
+            b = torch.as_tensor(values).to(self.device, torch.uint8).reshape(-1).contiguous()
+            off = self._offsets(offsets)
+        else:
+            b, off = self._pack([np.frombuffer(bytes(s), dtype=np.uint8) for s in x], np.uint8)
+        self._call(N.lib.cpb_poseidon_duplex_absorb_bytes_ragged_dev, b, off)
+
+    def fork(self, domains) -> "RaggedPoseidonSpongeBatch":
+        """R/sponge/mod.rs:145-153 for every sponge with its own domain: clone, then sponge i absorbs the byte string
+        usize(len(domains[i])) || domains[i]."""
+        new = self.clone()
+        new.absorb_bytes([len(d).to_bytes(8, "little") + bytes(d) for d in domains])
+        return new
+
+    # -- squeeze
+    def _squeeze(self, counts, canonical: bool):
+        import torch
+        if isinstance(counts, int):
+            if counts < 0:
+                raise ValueError("counts must not be negative")
+            off = torch.arange(self.n + 1, dtype=torch.int64, device=self.device) * counts
+            total = self.n * counts
+        else:
+            c = torch.as_tensor(counts, dtype=torch.int64).to(self.device).reshape(-1)
+            if c.shape[0] != self.n:
+                raise ValueError(f"expected {self.n} counts (got {c.shape[0]})")
+            if self.n and int(c.min()) < 0:
+                raise ValueError("counts must not be negative")
+            off = torch.zeros(self.n + 1, dtype=torch.int64, device=self.device)
+            torch.cumsum(c, 0, out=off[1:])
+            total = int(off[-1]) if self.n else 0
+        out = torch.empty((total, 4), dtype=torch.int64, device=self.device)
+        self._call(N.lib.cpb_poseidon_duplex_squeeze_ragged_dev, out, off, int(canonical))
+        return out, off
+
+    def squeeze_native_field_elements(self, counts):
+        """Sponge i squeezes counts[i] (or counts, an int, for all) native elements: (values (S, 4) Montgomery limbs, offsets (n + 1)),
+        torch int64 on the device; sponge i's are values[offsets[i] .. offsets[i+1])."""
+        return self._squeeze(counts, False)
+
+    def squeeze_canonical(self, counts):
+        """squeeze_native_field_elements as canonical integers (little-endian limbs)."""
+        return self._squeeze(counts, True)
 
 
 def _cuda_device(device):

@@ -78,7 +78,8 @@ const char* cpb_last_error(void);
 
 /* ABI revision of this header: bumped when entry points or status codes are added (2 = CPB_INTERNAL_ERROR, cpb_abi_version; 3 = _dev field conversion, host pinning, launch count, multi-GPU build, CPB_NCCL_ERROR, wire formats; 4 = ragged Poseidon batches: CRH, sponge, Merkle build and path verification over inputs of different lengths; 5 = Merkle update and
  * check_update of Poseidon-node trees, in place on device arrays or over host arrays; later additions under 5 are additive: Merkle path verification of the Pedersen
- * trees, batched duplex sponges with the cpb_sponge_mode type). */
+ * trees, batched duplex sponges with the cpb_sponge_mode type, ragged duplex calls with a mode per sponge -- a library that has
+ * them exports cpb_poseidon_duplex_absorb_ragged). */
 #define CPB_ABI_VERSION 5
 int cpb_abi_version(void);
 int cpb_version(void);
@@ -182,6 +183,40 @@ cpb_status cpb_poseidon_duplex_squeeze(cpb_poseidon_ctx* ctx, uint64_t* states, 
                                        int canonical, size_t n);
 cpb_status cpb_poseidon_duplex_squeeze_dev(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* mode, uint64_t* out, size_t m,
                                            int canonical, size_t n, void* stream);
+/* Ragged duplex calls: n sponges with a mode EACH, modes[i] (n cpb_sponge_mode), and a span each under the layout of the ragged
+ * batches below: offsets holds n + 1 uint64_t and sponge i's span is buf[offsets[i] .. offsets[i+1]), in elements (field data) or
+ * in bytes (byte strings); offsets[0] need not be 0.  Every sponge follows the reference's rules from its own mode and gets its new
+ * mode written back:
+ *   absorb_ragged         sponge i absorbs the native elements of its span of `values`;
+ *   absorb_bytes_ragged   sponge i absorbs its span of `bytes` as one [u8] value (its own 8-byte length, then 31-byte chunks),
+ *                         as cpb_poseidon_duplex_absorb_bytes does for that string;
+ *   squeeze_ragged        sponge i runs squeeze_native_field_elements(offsets[i+1] - offsets[i]) into its span of `out`, as
+ *                         Montgomery limbs or (canonical != 0) canonical integers; 0 elements still permute from Absorbing mode.
+ * The mode layout: 16 bytes, squeezing in bytes 0..3 (bytes 4..7 are padding and are not read), index at byte 8.  A written mode
+ * has its first 8-byte word whole, padding zeroed, so an int64 array of (n, 2) holds [squeezing, index] per row.
+ * Argument checks, before any device work, in this order: n >= 2^32 -> CPB_BAD_LENGTH; n == 0 -> CPB_OK, nothing launched;
+ * states, modes or offsets NULL -> CPB_NULL_POINTER.  Host forms then: decreasing offsets -> CPB_BAD_LENGTH; a NULL data buffer
+ * while the spans are not all empty -> CPB_NULL_POINTER; a mode with squeezing not 0 or 1 -> CPB_BAD_PARAMS.  Then ctx NULL ->
+ * CPB_NULL_POINTER, and for host forms a mode with index > rate -> CPB_BAD_PARAMS.  On an error states, modes and outputs are
+ * unchanged.  Spans are clamped as in the ragged batches: a decreasing pair is an empty span, and nothing outside
+ * [offsets[0], offsets[n]) is read or written.
+ * Host forms: host arrays; only buf[offsets[0] .. offsets[n]) is copied, indexed from offsets[0]; one host synchronisation.
+ * _dev forms: every array is device memory and the modes are updated in place; nothing in device memory is checked.  A sponge
+ * whose mode is invalid (squeezing, read from bytes 0..3, not 0 or 1, or index > rate) is left untouched -- state and mode as they
+ * were -- and its squeeze span is written as zeros; the other sponges are unaffected.  The device sorts the sponges by their
+ * permutation count first; scratch comes from the stream-ordered pool and nothing synchronises the host (CUDA-graph capturable). */
+cpb_status cpb_poseidon_duplex_absorb_ragged(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* modes, const uint64_t* values,
+                                             const uint64_t* offsets, size_t n);
+cpb_status cpb_poseidon_duplex_absorb_ragged_dev(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* modes, const uint64_t* values,
+                                                 const uint64_t* offsets, size_t n, void* stream);
+cpb_status cpb_poseidon_duplex_absorb_bytes_ragged(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* modes, const uint8_t* bytes,
+                                                   const uint64_t* offsets, size_t n);
+cpb_status cpb_poseidon_duplex_absorb_bytes_ragged_dev(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* modes, const uint8_t* bytes,
+                                                       const uint64_t* offsets, size_t n, void* stream);
+cpb_status cpb_poseidon_duplex_squeeze_ragged(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* modes, uint64_t* out,
+                                              const uint64_t* offsets, int canonical, size_t n);
+cpb_status cpb_poseidon_duplex_squeeze_ragged_dev(cpb_poseidon_ctx* ctx, uint64_t* states, cpb_sponge_mode* modes, uint64_t* out,
+                                                  const uint64_t* offsets, int canonical, size_t n, void* stream);
 
 /* ---- Merkle tree, field leaves ---------------------------------------------------------- */
 /* MerkleTree::new (R/merkle_tree/mod.rs:411-422) for Config{Leaf=[F], LeafDigest=InnerDigest=F,

@@ -173,6 +173,56 @@ private:
     cpb_sponge_mode mode_;
 };
 
+// n PoseidonSponge<F> over one Config with a DuplexSpongeMode each, so every call can give each sponge a different number of
+// elements: one cpb_poseidon_duplex_*_ragged call for the batch.  Ragged data is (buffer, offsets): offsets has n + 1 entries and
+// sponge i's part is buffer[offsets[i] .. offsets[i+1]).  States are host memory (n x t elements, Montgomery); the Config must
+// outlive the batch.
+class RaggedPoseidonSpongeBatch {
+public:
+    RaggedPoseidonSpongeBatch(const Config& p, size_t n)
+        : p_(&p), n_(n), states_(n * (size_t)(p.rate + p.capacity), Fe{0, 0, 0, 0}), modes_(n, cpb_sponge_mode{0, 0}) {}
+    // a copy of a uniform batch: its states, and its one mode for every sponge
+    RaggedPoseidonSpongeBatch(const Config& p, const PoseidonSpongeBatch& b)
+        : p_(&p), n_(b.size()), states_(b.states()), modes_(b.size(), b.mode()) {}
+
+    // sponge i absorbs values[offsets[i] .. offsets[i+1])
+    void absorb(const std::vector<Fe>& values, const std::vector<uint64_t>& offsets) {
+        check_offsets(offsets, values.size());
+        check(cpb_poseidon_duplex_absorb_ragged(p_->ctx(), data(), mode_ptr(), values.empty() ? nullptr : values[0].data(), offsets.data(), n_));
+    }
+    // sponge i absorbs the byte string bytes[offsets[i] .. offsets[i+1]) as one [u8] value (R/sponge/absorb.rs:137-141)
+    void absorb_bytes(const std::vector<uint8_t>& bytes, const std::vector<uint64_t>& offsets) {
+        check_offsets(offsets, bytes.size());
+        check(cpb_poseidon_duplex_absorb_bytes_ragged(p_->ctx(), data(), mode_ptr(), bytes.empty() ? nullptr : bytes.data(), offsets.data(), n_));
+    }
+    // sponge i runs squeeze_native_field_elements(offsets[i+1] - offsets[i]) into out[offsets[i] ..]; out has offsets[n] elements
+    // (Montgomery limbs, or canonical integers)
+    std::vector<Fe> squeeze(const std::vector<uint64_t>& offsets, bool canonical) {
+        check_offsets(offsets, (size_t)-1);
+        std::vector<Fe> out(offsets.empty() ? 0 : offsets.back());
+        check(cpb_poseidon_duplex_squeeze_ragged(p_->ctx(), data(), mode_ptr(), out.empty() ? nullptr : out[0].data(), offsets.data(),
+                                                 canonical ? 1 : 0, n_));
+        return out;
+    }
+
+    size_t size() const { return n_; }
+    const std::vector<Fe>& states() const { return states_; }    // sponge i's state at [i * t ..]
+    const std::vector<cpb_sponge_mode>& modes() const { return modes_; }
+
+private:
+    void check_offsets(const std::vector<uint64_t>& offsets, size_t len) const {
+        if (offsets.size() != n_ + 1) throw Error(CPB_BAD_LENGTH, "ragged call: offsets needs n + 1 entries");
+        for (uint64_t o : offsets)
+            if (o > len) throw Error(CPB_BAD_LENGTH, "ragged call: an offset lies past the buffer");
+    }
+    uint64_t* data() { return states_.empty() ? nullptr : states_[0].data(); }
+    cpb_sponge_mode* mode_ptr() { return modes_.empty() ? nullptr : modes_.data(); }
+    const Config* p_;
+    size_t n_;
+    std::vector<Fe> states_;
+    std::vector<cpb_sponge_mode> modes_;
+};
+
 }  // namespace poseidon
 
 namespace pedersen {
