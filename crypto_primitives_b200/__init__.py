@@ -7,7 +7,7 @@ interface plus ctypes plumbing.  There is no CPU fallback: importing fails witho
 and every compute call fails without an H100.
 """
 from . import _native
-from .fields import BLS12_381_FR, BLS12_377_FR, BN254_FR, JUBJUB_FR, FIELDS, Field
+from .fields import BLS12_381_FR, BLS12_377_FR, BN254_FR, ED_ON_BLS12_377_FR, JUBJUB_FR, FIELDS, Field
 from .sponge.poseidon import (PoseidonConfig, PoseidonSponge, PoseidonSpongeBatch, RaggedPoseidonSpongeBatch, absorb_squeeze_batch, absorb_squeeze_ragged, find_poseidon_ark_and_mds,
                               get_default_poseidon_parameters)
 from .crh import poseidon as crh_poseidon
@@ -22,7 +22,7 @@ from .encryption.elgamal import ElGamal
 from . import curves
 from . import merkle_tree
 
-__all__ = ["Field", "FIELDS", "BLS12_381_FR", "BN254_FR", "JUBJUB_FR", "BLS12_377_FR", "PoseidonConfig", "PoseidonSponge", "PoseidonSpongeBatch", "RaggedPoseidonSpongeBatch", "absorb_squeeze_batch",
+__all__ = ["Field", "FIELDS", "BLS12_381_FR", "BN254_FR", "JUBJUB_FR", "BLS12_377_FR", "ED_ON_BLS12_377_FR", "PoseidonConfig", "PoseidonSponge", "PoseidonSpongeBatch", "RaggedPoseidonSpongeBatch", "absorb_squeeze_batch",
            "absorb_squeeze_ragged",
            "find_poseidon_ark_and_mds", "get_default_poseidon_parameters", "crh_poseidon", "crh_pedersen", "crh_bowe_hopwood", "commitment_pedersen",
            "commitment_blake2s", "signature_schnorr", "Schnorr", "encryption_elgamal", "ElGamal", "curves", "merkle_tree"]

@@ -145,6 +145,7 @@ SIGNATURES = {
     "cpb_multi_uses_nccl": (C.c_int, [vp]),
     "cpb_merkle_poseidon_build_multi": (C.c_int, [vp, C.POINTER(vp), C.POINTER(vp), u64p, C.c_size_t, C.c_size_t, u64p, u64p]),
     "cpb_te_base_ctx_create": (C.c_int, [C.c_int, u64p, C.c_int, C.POINTER(vp)]),
+    "cpb_te_base_ctx_create_ex": (C.c_int, [C.c_int, u64p, C.c_int, C.POINTER(vp)]),
     "cpb_te_base_ctx_destroy": (None, [vp]),
     "cpb_te_base_mul_batch": (C.c_int, [vp, u64p, u64p, C.c_size_t]),
     "cpb_te_base_mul_batch_dev": (C.c_int, [vp, vp, vp, C.c_size_t, vp]),

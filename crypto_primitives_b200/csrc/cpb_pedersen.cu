@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "curve_desc.hpp"
 #include "hostfp.hpp"
 #include "pedersen.cuh"
 #include "pedersen_internal.cuh"
@@ -497,18 +498,6 @@ extern "C" int cpb_poseidon_ctx_device(const cpb_poseidon_ctx* ctx);
 namespace {
 
 
-struct CurveInfo {
-    int field_id;
-    bool d_is_ratio;      // d = -(num/den) when true, else d = num
-    uint64_t num, den;
-};
-bool curve_info(int curve_id, CurveInfo& ci) {
-    switch (curve_id) {
-        case CPB_JUBJUB: ci = {CPB_BLS12_381_FR, true, 10240, 10241}; return true;          // ark-ed-on-bls12-381: a=-1, d=-(10240/10241)
-        case CPB_ED_ON_BLS12_377: ci = {CPB_BLS12_377_FR, false, 3021, 1}; return true;     // ark-ed-on-bls12-377: a=-1, d=3021
-    }
-    return false;
-}
 
 template <class K> cpb_status ped_grid(K kernel, size_t smem, int sms, long n, int& grid) {
     static thread_local const void* last = nullptr;
@@ -650,14 +639,14 @@ cpb_status cpb_pedersen_ctx_create_ex(int curve_id, int window_size, int num_win
     }
     if (chunk_bits < 8 || chunk_bits > 22) return fail(CPB_BAD_PARAMS, "chunk_bits must be 8..22 (0 = default)");
     *out = nullptr;
-    CurveInfo ci;
-    if (!curve_info(curve_id, ci)) return fail(CPB_BAD_PARAMS, "unknown curve id %d", curve_id);
+    host::CurveDesc ci;
+    if (!host::curve_desc(curve_id, ci)) return fail(CPB_BAD_PARAMS, "unknown curve id %d", curve_id);
     if (window_size < 1 || num_windows < 1 || (size_t)window_size * num_windows > (1u << 20))
         return fail(CPB_BAD_PARAMS, "bad window %dx%d", window_size, num_windows);
     if (!generators_xy || (n_rand && !rand_generators_xy)) return fail(CPB_NULL_POINTER, "null generators");
     if (n_rand > 256) return fail(CPB_BAD_PARAMS, "at most 256 randomness generators");
     host::Field F(host::field_modulus(ci.field_id));
-    host::Fe d = ci.d_is_ratio ? F.neg(F.mul(F.from_u64(ci.num), F.inv(F.from_u64(ci.den)))) : F.from_u64(ci.num);
+    host::Fe d = ci.d(F);
     host::Fe d2 = F.add(d, d);
     const size_t nbits = (size_t)window_size * num_windows;
     auto on_curve = [&](const uint64_t* xy) {
@@ -1019,13 +1008,13 @@ cpb_status cpb_bowe_hopwood_ctx_create(int curve_id, int window_size, int num_wi
     return cpb::guarded([&]() -> cpb_status {
     if (!out) return fail(CPB_NULL_POINTER, "null out");
     *out = nullptr;
-    CurveInfo ci;
-    if (!curve_info(curve_id, ci)) return fail(CPB_BAD_PARAMS, "unknown curve id %d", curve_id);
+    host::CurveDesc ci;
+    if (!host::curve_desc(curve_id, ci)) return fail(CPB_BAD_PARAMS, "unknown curve id %d", curve_id);
     if (window_size < 1 || num_windows < 1 || (size_t)window_size * num_windows > (1u << 16))
         return fail(CPB_BAD_PARAMS, "bad window %dx%d", window_size, num_windows);
     if (!generators_xy) return fail(CPB_NULL_POINTER, "null generators");
     host::Field F(host::field_modulus(ci.field_id));
-    host::Fe d = ci.d_is_ratio ? F.neg(F.mul(F.from_u64(ci.num), F.inv(F.from_u64(ci.den)))) : F.from_u64(ci.num);
+    host::Fe d = ci.d(F);
     host::Fe d2 = F.add(d, d);
     const size_t n_gens = (size_t)window_size * num_windows;
     for (size_t i = 0; i < n_gens; i++) {

@@ -76,8 +76,10 @@ __global__ void k_field_convert(const u32* __restrict__ in, u32* __restrict__ ou
     u32 a[8], k[8];
     ld_elem(a, in + 8 * i);
     if (to_mont) {
-        // inputs < 2^256 may exceed p: subtract p while >= p (at most 6 times for a 252-bit p... bounded loop)
-        for (int it = 0; it < 18; it++) {
+        // inputs < 2^256 may exceed p: subtract p while >= p (bounded loop: 2^256 / p < 2^32 / p[7] subtractions, at most 17
+        // for the 252-bit and wider moduli, 54 for the 251-bit scalar field of ed-on-BLS12-377)
+        constexpr int kSubs = (int)((1ull << 32) / F::P(7)) + 1 > 18 ? (int)((1ull << 32) / F::P(7)) + 1 : 18;
+        for (int it = 0; it < kSubs; it++) {
             u32 t[8];
             t[0] = sub_cc(a[0], F::P(0));
 #pragma unroll
@@ -611,7 +613,7 @@ cpb_status cpb_host_unregister(void* ptr) {
 
 cpb_status cpb_field_modulus(int field_id, uint64_t out[4]) {
     return cpb::guarded([&]() -> cpb_status {
-    const uint64_t* m = host::field_modulus(field_id);
+    const uint64_t* m = host::element_field_modulus(field_id);
     if (!m) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
     if (!out) return fail(CPB_NULL_POINTER, "null out");
     memcpy(out, m, 32);
@@ -620,7 +622,7 @@ cpb_status cpb_field_modulus(int field_id, uint64_t out[4]) {
 }
 
 static cpb_status field_convert(int field_id, int device, const uint64_t* in, uint64_t* out, size_t n, int to_mont) {
-    if (!host::field_modulus(field_id)) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
+    if (!host::element_field_modulus(field_id)) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
     if (n == 0) return CPB_OK;
     if (!in || !out) return fail(CPB_NULL_POINTER, "null buffer");
     DeviceGuard g(device);
@@ -635,6 +637,7 @@ static cpb_status field_convert(int field_id, int device, const uint64_t* in, ui
             case 1: k_field_convert<Bn254_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
             case 2: k_field_convert<Jubjub_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
             case 3: k_field_convert<Bls12_377_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
+            case 4: k_field_convert<Ed_On_Bls12_377_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
         }
         e = cudaGetLastError();
     }
@@ -644,7 +647,7 @@ static cpb_status field_convert(int field_id, int device, const uint64_t* in, ui
     return CPB_OK;
 }
 static cpb_status field_convert_dev(int field_id, int device, const uint64_t* in, uint64_t* out, size_t n, int to_mont, void* stream) {
-    if (!host::field_modulus(field_id)) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
+    if (!host::element_field_modulus(field_id)) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
     if (n == 0) return CPB_OK;
     if (!in || !out) return fail(CPB_NULL_POINTER, "null buffer");
     DeviceGuard g(device);
@@ -661,6 +664,7 @@ static cpb_status field_convert_dev(int field_id, int device, const uint64_t* in
             case 1: k_field_convert<Bn254_Fr><<<grid, 128, 0, st>>>(d_in + 8 * off, d_out + 8 * off, m, to_mont); break;
             case 2: k_field_convert<Jubjub_Fr><<<grid, 128, 0, st>>>(d_in + 8 * off, d_out + 8 * off, m, to_mont); break;
             case 3: k_field_convert<Bls12_377_Fr><<<grid, 128, 0, st>>>(d_in + 8 * off, d_out + 8 * off, m, to_mont); break;
+            case 4: k_field_convert<Ed_On_Bls12_377_Fr><<<grid, 128, 0, st>>>(d_in + 8 * off, d_out + 8 * off, m, to_mont); break;
         }
         CPB_CUDA(cudaGetLastError());
         left -= m; off += m;

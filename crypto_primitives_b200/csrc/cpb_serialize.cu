@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "curve_desc.hpp"
 #include "hostfp.hpp"
 
 using namespace cpb;
@@ -26,23 +27,8 @@ typedef host::u64 hu64;
 
 namespace {
 
-struct CurveDesc {
-    int field_id;
-    bool d_is_ratio;
-    hu64 num, den;            // d = -(num/den) when d_is_ratio else num; a = -1
-    hu64 order[4];            // prime subgroup order (scalar-field modulus)
-};
-bool curve_desc(int curve_id, CurveDesc& c) {
-    switch (curve_id) {
-        case CPB_JUBJUB:
-            c = {CPB_BLS12_381_FR, true, 10240, 10241, {0xd0970e5ed6f72cb7ull, 0xa6682093ccc81082ull, 0x06673b0101343b00ull, 0x0e7db4ea6533afa9ull}};
-            return true;
-        case CPB_ED_ON_BLS12_377:
-            c = {CPB_BLS12_377_FR, false, 3021, 1, {0xb95aee9ac33fd9ffull, 0x5293a3afc43c8afeull, 0x982d1347970dec00ull, 0x04aad957a68b2955ull}};
-            return true;
-    }
-    return false;
-}
+using host::CurveDesc;
+using host::curve_desc;
 
 size_t fbytes(const Field& F) { return (size_t)(F.bits + 7) / 8; }
 
@@ -153,7 +139,7 @@ struct Curve {
     Fe d;
     CurveDesc desc;
     explicit Curve(const CurveDesc& c) : F(host::field_modulus(c.field_id)), desc(c) {
-        d = c.d_is_ratio ? F.neg(F.mul(F.from_u64(c.num), F.inv(F.from_u64(c.den)))) : F.from_u64(c.num);
+        d = c.d(F);
     }
     bool on_curve(const Fe& x, const Fe& y) const {
         Fe xx = F.mul(x, x), yy = F.mul(y, y);
@@ -169,8 +155,9 @@ struct Curve {
     }
     bool in_subgroup(const Fe& x, const Fe& y) const {
         Pt acc{F.zero(), F.one(), F.one(), F.zero()}, base{x, y, F.one(), F.mul(x, y)};
+        const hu64* order = desc.order();
         for (int i = 0; i < 256; i++) {
-            if ((desc.order[i / 64] >> (i % 64)) & 1) acc = add(acc, base);
+            if ((order[i / 64] >> (i % 64)) & 1) acc = add(acc, base);
             base = add(base, base);
         }
         return acc.X.is_zero() && acc.Y == acc.Z;        // (0 : 1 : 1)
@@ -244,14 +231,14 @@ struct Codec {
 extern "C" {
 
 size_t cpb_field_serialized_size(int field_id) {
-    const hu64* m = host::field_modulus(field_id);
+    const hu64* m = host::element_field_modulus(field_id);
     if (!m) return 0;
     return fbytes(Field(m));
 }
 
 cpb_status cpb_field_serialize(int field_id, const uint64_t* mont, size_t n, uint8_t* out) {
     return cpb::guarded([&]() -> cpb_status {
-    const hu64* m = host::field_modulus(field_id);
+    const hu64* m = host::element_field_modulus(field_id);
     if (!m) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
     if (n && (!mont || !out)) return fail(CPB_NULL_POINTER, "null buffer");
     Field F(m);
@@ -263,7 +250,7 @@ cpb_status cpb_field_serialize(int field_id, const uint64_t* mont, size_t n, uin
 }
 cpb_status cpb_field_deserialize(int field_id, const uint8_t* in, size_t n, uint64_t* mont_out) {
     return cpb::guarded([&]() -> cpb_status {
-    const hu64* m = host::field_modulus(field_id);
+    const hu64* m = host::element_field_modulus(field_id);
     if (!m) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
     if (n && (!in || !mont_out)) return fail(CPB_NULL_POINTER, "null buffer");
     Field F(m);

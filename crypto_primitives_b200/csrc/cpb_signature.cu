@@ -1,5 +1,6 @@
 // cpb_signature.cu -- CUDA kernels + C-ABI for Schnorr signatures (R/signature/schnorr/mod.rs), ElGamal encryption
-// (R/encryption/elgamal/mod.rs) over Jubjub, and the Blake2s commitment (R/commitment/blake2s/mod.rs); include/cpb200.h.
+// (R/encryption/elgamal/mod.rs) over Jubjub and ed-on-BLS12-377, and the Blake2s commitment (R/commitment/blake2s/mod.rs);
+// include/cpb200.h.
 //
 // Fixed-base products s*G run on the Pedersen table machinery: the context owns a Pedersen context whose 256 generators
 // are 2^k G (window 256 x 1), and hashing the 32-byte little-endian canonical scalar selects exactly the generators of
@@ -12,6 +13,7 @@
 //   k_elgamal_encrypt      c2 = r*pk + m (c1 = r*G from the tables)
 //   k_elgamal_decrypt      c2 - sk*c1
 //   k_blake2s_commit       Blake2s(input || r)
+// Every kernel but the commitment is a template on the curve (SigCurve below); a context dispatches on its curve id.
 // A call issues several launches on one stream and never synchronises the host; scratch comes from the stream-ordered
 // pool.  Secret scalars index tables with data-dependent indices: this code is not constant time (nor is the reference's).
 #include <cstring>
@@ -19,15 +21,24 @@
 
 #include "blake2s.cuh"
 #include "common.cuh"
+#include "curve_desc.hpp"
 #include "hostfp.hpp"
 #include "te_ops.cuh"
 
 namespace cpb {
 
-typedef Bls12_381_Fr JqF;      // Jubjub base field
-typedef Jubjub_Fr JrF;         // Jubjub scalar field
+// A curve of the signature layer: base field Fq and scalar field Fr as device field tags, with their C-ABI ids.
+template <class Q, class R, int CURVE, int FQ_ID, int FR_ID> struct SigCurve {
+    typedef Q Fq;
+    typedef R Fr;
+    static constexpr int kCurve = CURVE, kFqId = FQ_ID, kFrId = FR_ID;
+    static constexpr int kFrNibbles = (R::BITS + 3) / 4;   // nibbles of a canonical scalar (below r < 2^BITS)
+    static_assert(Q::ID == FQ_ID && R::ID == FR_ID, "field tags and ids disagree");
+};
+typedef SigCurve<Bls12_381_Fr, Jubjub_Fr, CPB_JUBJUB, CPB_BLS12_381_FR, CPB_JUBJUB_FR> JubjubSig;                     // r < 2^252: 63
+typedef SigCurve<Bls12_377_Fr, Ed_On_Bls12_377_Fr, CPB_ED_ON_BLS12_377, CPB_BLS12_377_FR, CPB_ED_ON_BLS12_377_FR> Ed377Sig;  // r < 2^251: 63
+static_assert(JubjubSig::kFrNibbles == 63 && Ed377Sig::kFrNibbles == 63, "te_mul_var digit count");
 constexpr int kSigBlock = 128;
-constexpr int kFrNibbles = 63;  // canonical Fr scalars are below r < 2^252
 
 struct Salt {
     u32 w[8];
@@ -50,25 +61,27 @@ __device__ __forceinline__ void msg_range(const u64* off, long i, u64& start, u6
     len = b > a ? b - a : 0;                             // a decreasing pair hashes as an empty message
 }
 
-__device__ __forceinline__ void affine_add(TePoint& acc, const u32* x, const u32* y, const SigConsts& c) {
+template <class C> __device__ __forceinline__ void affine_add(TePoint& acc, const u32* x, const u32* y, const SigConsts& c) {
     u32 yp[8], ym[8], t2d[8];
-    te_niels<JqF>(yp, ym, t2d, x, y, c.d2, c.pm);
-    te_madd<JqF>(acc, yp, ym, t2d, c.pm);
+    te_niels<typename C::Fq>(yp, ym, t2d, x, y, c.d2, c.pm);
+    te_madd<typename C::Fq>(acc, yp, ym, t2d, c.pm);
 }
 
 // Schnorr challenge: from_random_bytes(Blake2s256(salt || compress(R) || u64_le(len) || msg)), R affine
+template <class C>
 __device__ __forceinline__ bool schnorr_challenge(u32* e, const Salt& salt, const u32* rx, const u32* ry, const uint8_t* msg,
                                                   u64 len, const SigConsts& c) {
     u32 hdr[18], dg[8];
 #pragma unroll
     for (int i = 0; i < 8; i++) hdr[i] = salt.w[i];
-    te_compress<JqF>(hdr + 8, rx, ry, c.pm);
+    te_compress<typename C::Fq>(hdr + 8, rx, ry, c.pm);
     hdr[16] = (u32)len;
     hdr[17] = (u32)(len >> 32);
     blake2s_256(dg, B2sSchnorr{hdr, msg}, 72 + len);
-    return fr_from_random_bytes<JrF>(e, dg, c.sm);
+    return fr_from_random_bytes<typename C::Fr>(e, dg, c.sm);
 }
 
+template <class C>
 __global__ void __launch_bounds__(kSigBlock)
 k_fr_to_bytes(const u32* __restrict__ consts, const u32* __restrict__ sc, int stride_words, u32* __restrict__ out, long n, int zero) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -77,10 +90,11 @@ k_fr_to_bytes(const u32* __restrict__ consts, const u32* __restrict__ sc, int st
     ld_consts(c, consts, zero);
     u32 a[8];
     ld_elem(a, sc + stride_words * i);
-    fp_to_canonical<JrF>(a, a, c.sm);
+    fp_to_canonical<typename C::Fr>(a, a, c.sm);
     st_elem(out + 8 * i, a);
 }
 
+template <class C>
 __global__ void __launch_bounds__(kSigBlock)
 k_schnorr_sign(const u32* __restrict__ consts, Salt salt, const u32* __restrict__ r_xy, const u32* __restrict__ nonces,
                const u32* __restrict__ sks, const uint8_t* __restrict__ msgs, const u64* __restrict__ off, u32* __restrict__ sigs,
@@ -94,13 +108,13 @@ k_schnorr_sign(const u32* __restrict__ consts, Salt salt, const u32* __restrict_
     ld_elem(ry, r_xy + 16 * i + 8);
     u64 start, len;
     msg_range(off, i, start, len);
-    const bool ok = schnorr_challenge(e, salt, rx, ry, msgs + start, len, c);
+    const bool ok = schnorr_challenge<C>(e, salt, rx, ry, msgs + start, len, c);
     if (ok) {
         u32 k[8], sk[8];
         ld_elem(k, nonces + 8 * i);
         ld_elem(sk, sks + 8 * i);
-        fp_mul<JrF>(s, e, sk, c.sm);
-        fp_sub<JrF>(s, k, s);                            // prover_response = k - e*sk (mod.rs:106)
+        fp_mul<typename C::Fr>(s, e, sk, c.sm);
+        fp_sub<typename C::Fr>(s, k, s);                            // prover_response = k - e*sk (mod.rs:106)
     } else {
         fp_zero(s);
         fp_zero(e);
@@ -110,6 +124,7 @@ k_schnorr_sign(const u32* __restrict__ consts, Salt salt, const u32* __restrict_
     signed_out[i] = ok ? 1 : 0;
 }
 
+template <class C>
 __global__ void __launch_bounds__(kSigBlock)
 k_schnorr_verify(const u32* __restrict__ consts, Salt salt, const u32* __restrict__ sg_xy, const u32* __restrict__ pks,
                  const uint8_t* __restrict__ msgs, const u64* __restrict__ off, const u32* __restrict__ sigs, uint8_t* __restrict__ ok_out,
@@ -120,23 +135,24 @@ k_schnorr_verify(const u32* __restrict__ consts, Salt salt, const u32* __restric
     ld_consts(c, consts, zero);
     u32 e[8], x[8], y[8];
     ld_elem(e, sigs + 16 * i + 8);
-    fp_to_canonical<JrF>(e, e, c.sm);
+    fp_to_canonical<typename C::Fr>(e, e, c.sm);
     ld_elem(x, pks + 16 * i);
     ld_elem(y, pks + 16 * i + 8);
     TePoint acc;
-    te_mul_var<JqF>(acc, x, y, ScalarWords{e, kFrNibbles}, c.d2, c.pm);      // e*pk
+    te_mul_var<typename C::Fq>(acc, x, y, ScalarWords{e, C::kFrNibbles}, c.d2, c.pm);      // e*pk
     ld_elem(x, sg_xy + 16 * i);
     ld_elem(y, sg_xy + 16 * i + 8);
-    affine_add(acc, x, y, c);                                                  // + s*G (mod.rs:124-127)
-    te_to_affine<JqF>(x, y, acc, c.pm);
+    affine_add<C>(acc, x, y, c);                                                  // + s*G (mod.rs:124-127)
+    te_to_affine<typename C::Fq>(x, y, acc, c.pm);
     u64 start, len;
     msg_range(off, i, start, len);
     u32 e2[8];
-    const bool valid = schnorr_challenge(e2, salt, x, y, msgs + start, len, c);
+    const bool valid = schnorr_challenge<C>(e2, salt, x, y, msgs + start, len, c);
     ld_elem(e, sigs + 16 * i + 8);
     ok_out[i] = valid && fp_eq(e, e2) ? 1 : 0;
 }
 
+template <class C>
 __global__ void __launch_bounds__(kSigBlock)
 k_schnorr_rand_pk(const u32* __restrict__ consts, const u32* __restrict__ pks, const uint8_t* __restrict__ rnd, long len, long stride,
                   u32* __restrict__ out, long n, int zero) {
@@ -148,15 +164,16 @@ k_schnorr_rand_pk(const u32* __restrict__ consts, const u32* __restrict__ pks, c
     ld_elem(gx, consts + 24);
     ld_elem(gy, consts + 32);
     TePoint acc;
-    te_mul_var<JqF>(acc, gx, gy, ScalarBitrevBytes{rnd + i * stride, (u64)len}, c.d2, c.pm);
+    te_mul_var<typename C::Fq>(acc, gx, gy, ScalarBitrevBytes{rnd + i * stride, (u64)len}, c.d2, c.pm);
     ld_elem(x, pks + 16 * i);
     ld_elem(y, pks + 16 * i + 8);
-    affine_add(acc, x, y, c);
-    te_to_affine<JqF>(x, y, acc, c.pm);
+    affine_add<C>(acc, x, y, c);
+    te_to_affine<typename C::Fq>(x, y, acc, c.pm);
     st_elem(out + 16 * i, x);
     st_elem(out + 16 * i + 8, y);
 }
 
+template <class C>
 __global__ void __launch_bounds__(kSigBlock)
 k_schnorr_rand_sig(const u32* __restrict__ consts, const u32* __restrict__ sigs, const uint8_t* __restrict__ rnd, long len, long stride,
                    u32* __restrict__ out, long n, int zero) {
@@ -166,28 +183,29 @@ k_schnorr_rand_sig(const u32* __restrict__ consts, const u32* __restrict__ sigs,
     ld_consts(c, consts, zero);
     u32 r2[8], c256[8], m[8], v[8], s[8], e[8];
 #pragma unroll
-    for (int k = 0; k < 8; k++) r2[k] = JrF::R2(k);
+    for (int k = 0; k < 8; k++) r2[k] = C::Fr::R2(k);
     fp_zero(c256);
     c256[0] = 256;
-    fp_mul<JrF>(c256, c256, r2, c.sm);
+    fp_mul<typename C::Fr>(c256, c256, r2, c.sm);
     fp_zero(m);
     const uint8_t* p = rnd + i * stride;
 #pragma unroll 1
     for (long b = len - 1; b >= 0; b--) {                // multiplier = sum_b bitrev8(byte_b) 256^b in Fr (mod.rs:161-168)
-        fp_mul<JrF>(m, m, c256, c.sm);
+        fp_mul<typename C::Fr>(m, m, c256, c.sm);
         fp_zero(v);
         v[0] = bitrev8(p[b]);
-        fp_mul<JrF>(v, v, r2, c.sm);
-        fp_add<JrF>(m, m, v);
+        fp_mul<typename C::Fr>(v, v, r2, c.sm);
+        fp_add<typename C::Fr>(m, m, v);
     }
     ld_elem(s, sigs + 16 * i);
     ld_elem(e, sigs + 16 * i + 8);
-    fp_mul<JrF>(m, e, m, c.sm);
-    fp_sub<JrF>(s, s, m);
+    fp_mul<typename C::Fr>(m, e, m, c.sm);
+    fp_sub<typename C::Fr>(s, s, m);
     st_elem(out + 16 * i, s);
     st_elem(out + 16 * i + 8, e);
 }
 
+template <class C>
 __global__ void __launch_bounds__(kSigBlock)
 k_elgamal_encrypt(const u32* __restrict__ consts, const u32* __restrict__ c1_xy, const u32* __restrict__ pks, const u32* __restrict__ ms,
                   const u32* __restrict__ rs, u32* __restrict__ out, long n, int zero) {
@@ -197,15 +215,15 @@ k_elgamal_encrypt(const u32* __restrict__ consts, const u32* __restrict__ c1_xy,
     ld_consts(c, consts, zero);
     u32 r[8], x[8], y[8];
     ld_elem(r, rs + 8 * i);
-    fp_to_canonical<JrF>(r, r, c.sm);
+    fp_to_canonical<typename C::Fr>(r, r, c.sm);
     ld_elem(x, pks + 16 * i);
     ld_elem(y, pks + 16 * i + 8);
     TePoint acc;
-    te_mul_var<JqF>(acc, x, y, ScalarWords{r, kFrNibbles}, c.d2, c.pm);      // s = r*pk
+    te_mul_var<typename C::Fq>(acc, x, y, ScalarWords{r, C::kFrNibbles}, c.d2, c.pm);      // s = r*pk
     ld_elem(x, ms + 16 * i);
     ld_elem(y, ms + 16 * i + 8);
-    affine_add(acc, x, y, c);                                                  // c2 = m + s
-    te_to_affine<JqF>(x, y, acc, c.pm);
+    affine_add<C>(acc, x, y, c);                                                  // c2 = m + s
+    te_to_affine<typename C::Fq>(x, y, acc, c.pm);
     st_elem(out + 32 * i + 16, x);
     st_elem(out + 32 * i + 24, y);
     ld_elem(x, c1_xy + 16 * i);
@@ -214,6 +232,7 @@ k_elgamal_encrypt(const u32* __restrict__ consts, const u32* __restrict__ c1_xy,
     st_elem(out + 32 * i + 8, y);
 }
 
+template <class C>
 __global__ void __launch_bounds__(kSigBlock)
 k_elgamal_decrypt(const u32* __restrict__ consts, const u32* __restrict__ sks, const u32* __restrict__ cts, u32* __restrict__ out, long n,
                   int zero) {
@@ -223,16 +242,16 @@ k_elgamal_decrypt(const u32* __restrict__ consts, const u32* __restrict__ sks, c
     ld_consts(c, consts, zero);
     u32 sk[8], x[8], y[8];
     ld_elem(sk, sks + 8 * i);
-    fp_to_canonical<JrF>(sk, sk, c.sm);
+    fp_to_canonical<typename C::Fr>(sk, sk, c.sm);
     ld_elem(x, cts + 32 * i);
     ld_elem(y, cts + 32 * i + 8);
     TePoint acc;
-    te_mul_var<JqF>(acc, x, y, ScalarWords{sk, kFrNibbles}, c.d2, c.pm);     // s = sk*c1
-    te_neg<JqF>(acc);
+    te_mul_var<typename C::Fq>(acc, x, y, ScalarWords{sk, C::kFrNibbles}, c.d2, c.pm);     // s = sk*c1
+    te_neg<typename C::Fq>(acc);
     ld_elem(x, cts + 32 * i + 16);
     ld_elem(y, cts + 32 * i + 24);
-    affine_add(acc, x, y, c);                                                  // m = c2 - s
-    te_to_affine<JqF>(x, y, acc, c.pm);
+    affine_add<C>(acc, x, y, c);                                                  // m = c2 - s
+    te_to_affine<typename C::Fq>(x, y, acc, c.pm);
     st_elem(out + 16 * i, x);
     st_elem(out + 16 * i + 8, y);
 }
@@ -316,38 +335,64 @@ Salt salt_of(const uint8_t* s) {
 }
 
 // s*G for n scalars read at sc + stride_words*i (Fr Montgomery) -> out_xy (n x 16 words), through the Pedersen tables.
-cpb_status base_mul_dev(cpb_te_base_ctx* c, const u32* sc, int stride_words, u32* out_xy, size_t n, cudaStream_t st) {
+template <class C> cpb_status base_mul_dev(cpb_te_base_ctx* c, const u32* sc, int stride_words, u32* out_xy, size_t n, cudaStream_t st) {
     PoolBuf bytes(st);
     CPB_TRY(bytes.alloc(32 * n));
-    k_fr_to_bytes<<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, sc, stride_words, bytes.as<u32>(), (long)n, 0);
+    k_fr_to_bytes<C><<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, sc, stride_words, bytes.as<u32>(), (long)n, 0);
     CPB_TRY(launched("k_fr_to_bytes"));
     return cpb_pedersen_crh_batch_dev(c->ped, bytes.as<uint8_t>(), 32, 32, (uint64_t*)out_xy, n, st);
 }
 
-cpb_status sign_dev(cpb_te_base_ctx* c, const Salt& salt, const u32* sks, const u32* nonces, const uint8_t* msgs, const u64* off,
+template <class C> cpb_status sign_dev(cpb_te_base_ctx* c, const Salt& salt, const u32* sks, const u32* nonces, const uint8_t* msgs, const u64* off,
                     u32* sigs, uint8_t* signed_out, size_t n, cudaStream_t st) {
     PoolBuf r(st);
     CPB_TRY(r.alloc(64 * n));
-    CPB_TRY(base_mul_dev(c, nonces, 8, r.as<u32>(), n, st));
-    k_schnorr_sign<<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, salt, r.as<u32>(), nonces, sks, msgs, off, sigs, signed_out, (long)n, 0);
+    CPB_TRY(base_mul_dev<C>(c, nonces, 8, r.as<u32>(), n, st));
+    k_schnorr_sign<C><<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, salt, r.as<u32>(), nonces, sks, msgs, off, sigs, signed_out, (long)n, 0);
     return launched("k_schnorr_sign");
 }
 
-cpb_status verify_dev(cpb_te_base_ctx* c, const Salt& salt, const u32* pks, const uint8_t* msgs, const u64* off, const u32* sigs,
+template <class C> cpb_status verify_dev(cpb_te_base_ctx* c, const Salt& salt, const u32* pks, const uint8_t* msgs, const u64* off, const u32* sigs,
                       uint8_t* ok, size_t n, cudaStream_t st) {
     PoolBuf sg(st);
     CPB_TRY(sg.alloc(64 * n));
-    CPB_TRY(base_mul_dev(c, sigs, 16, sg.as<u32>(), n, st));
-    k_schnorr_verify<<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, salt, sg.as<u32>(), pks, msgs, off, sigs, ok, (long)n, 0);
+    CPB_TRY(base_mul_dev<C>(c, sigs, 16, sg.as<u32>(), n, st));
+    k_schnorr_verify<C><<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, salt, sg.as<u32>(), pks, msgs, off, sigs, ok, (long)n, 0);
     return launched("k_schnorr_verify");
 }
 
-cpb_status encrypt_dev(cpb_te_base_ctx* c, const u32* pks, const u32* ms, const u32* rs, u32* out, size_t n, cudaStream_t st) {
+template <class C> cpb_status encrypt_dev(cpb_te_base_ctx* c, const u32* pks, const u32* ms, const u32* rs, u32* out, size_t n, cudaStream_t st) {
     PoolBuf c1(st);
     CPB_TRY(c1.alloc(64 * n));
-    CPB_TRY(base_mul_dev(c, rs, 8, c1.as<u32>(), n, st));
-    k_elgamal_encrypt<<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, c1.as<u32>(), pks, ms, rs, out, (long)n, 0);
+    CPB_TRY(base_mul_dev<C>(c, rs, 8, c1.as<u32>(), n, st));
+    k_elgamal_encrypt<C><<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, c1.as<u32>(), pks, ms, rs, out, (long)n, 0);
     return launched("k_elgamal_encrypt");
+}
+
+template <class C> cpb_status rand_pk_dev(cpb_te_base_ctx* c, const u32* pks, const uint8_t* rnd, size_t len, size_t stride, u32* out, size_t n,
+                                          cudaStream_t st) {
+    k_schnorr_rand_pk<C><<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, pks, rnd, (long)len, (long)stride, out, (long)n, 0);
+    return launched("k_schnorr_rand_pk");
+}
+
+template <class C> cpb_status rand_sig_dev(cpb_te_base_ctx* c, const u32* sigs, const uint8_t* rnd, size_t len, size_t stride, u32* out, size_t n,
+                                           cudaStream_t st) {
+    k_schnorr_rand_sig<C><<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, sigs, rnd, (long)len, (long)stride, out, (long)n, 0);
+    return launched("k_schnorr_rand_sig");
+}
+
+template <class C> cpb_status decrypt_dev(cpb_te_base_ctx* c, const u32* sks, const u32* cts, u32* out, size_t n, cudaStream_t st) {
+    k_elgamal_decrypt<C><<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, sks, cts, out, (long)n, 0);
+    return launched("k_elgamal_decrypt");
+}
+
+// fn(C{}) for the context's curve: every launch of a context runs that curve's kernel instances.
+template <class Fn> cpb_status on_curve(const cpb_te_base_ctx* c, Fn&& fn) {
+    switch (c->curve_id) {
+        case CPB_JUBJUB: return fn(JubjubSig{});
+        case CPB_ED_ON_BLS12_377: return fn(Ed377Sig{});
+    }
+    return fail(CPB_INTERNAL_ERROR, "context of curve %d", c->curve_id);
 }
 
 // Host-form plumbing: uploads on the context's stream, one synchronisation at the end.
@@ -390,7 +435,7 @@ struct HostCall {
     }
 };
 
-// Affine doubling over the host field (a = -1): x3 = 2xy / (1 + d x^2 y^2), y3 = (y^2 + x^2) / (1 - d x^2 y^2).
+// Affine doubling over the host field (a = -1, either curve): x3 = 2xy / (1 + d x^2 y^2), y3 = (y^2 + x^2) / (1 - d x^2 y^2).
 void host_double(const host::Field& F, const host::Fe& d, host::Fe& x, host::Fe& y) {
     host::Fe xx = F.mul(x, x), yy = F.mul(y, y), xy = F.mul(x, y);
     host::Fe k = F.mul(d, F.mul(xx, yy));
@@ -404,16 +449,27 @@ void host_double(const host::Field& F, const host::Fe& d, host::Fe& x, host::Fe&
 
 extern "C" {
 
+// The Jubjub-only form, with its contract unchanged: every other curve id is CPB_UNSUPPORTED, before the generator is read.
 cpb_status cpb_te_base_ctx_create(int curve_id, const uint64_t* generator_xy, int device, cpb_te_base_ctx** out) {
     return cpb::guarded([&]() -> cpb_status {
     if (!out) return fail(CPB_NULL_POINTER, "null out");
     *out = nullptr;
     if (curve_id != CPB_JUBJUB)
-        return fail(CPB_UNSUPPORTED, "curve %d: signatures and encryption need scalar-field arithmetic on the device, which exists for Jubjub only",
+        return fail(CPB_UNSUPPORTED, "curve %d: cpb_te_base_ctx_create is the Jubjub form; cpb_te_base_ctx_create_ex takes ed-on-BLS12-377",
                     curve_id);
+    return cpb_te_base_ctx_create_ex(curve_id, generator_xy, device, out);
+    });
+}
+
+cpb_status cpb_te_base_ctx_create_ex(int curve_id, const uint64_t* generator_xy, int device, cpb_te_base_ctx** out) {
+    return cpb::guarded([&]() -> cpb_status {
+    if (!out) return fail(CPB_NULL_POINTER, "null out");
+    *out = nullptr;
+    host::CurveDesc cd;
+    if (!host::curve_desc(curve_id, cd)) return fail(CPB_UNSUPPORTED, "curve %d: signatures and encryption exist for Jubjub and ed-on-BLS12-377", curve_id);
     if (!generator_xy) return fail(CPB_NULL_POINTER, "null generator");
-    host::Field F(host::field_modulus(CPB_BLS12_381_FR));
-    host::Fe d = F.neg(F.mul(F.from_u64(10240), F.inv(F.from_u64(10241))));
+    host::Field F(host::field_modulus(cd.field_id));
+    host::Fe d = cd.d(F);
     host::Fe x, y;
     memcpy(x.l, generator_xy, 32);
     memcpy(y.l, generator_xy + 4, 32);
@@ -435,13 +491,13 @@ cpb_status cpb_te_base_ctx_create(int curve_id, const uint64_t* generator_xy, in
     cpb_te_base_ctx* c = new cpb_te_base_ctx();
     c->curve_id = curve_id;
     c->device = device;
-    cpb_status st = cpb_pedersen_ctx_create_ex(CPB_JUBJUB, 256, 1, gens.data(), 0, nullptr, device, 0, &c->ped);
+    cpb_status st = cpb_pedersen_ctx_create_ex(curve_id, 256, 1, gens.data(), 0, nullptr, device, 0, &c->ped);
     if (st != CPB_OK) { delete c; return st; }
     host::Fe d2 = F.add(d, d);
     uint64_t consts[20];
     memcpy(consts, F.p, 32);
     memcpy(consts + 4, d2.l, 32);
-    memcpy(consts + 8, host::field_modulus(CPB_JUBJUB_FR), 32);
+    memcpy(consts + 8, cd.order(), 32);
     memcpy(consts + 12, generator_xy, 64);
     cudaError_t e = cudaMalloc(&c->d_consts, sizeof consts);
     if (e == cudaSuccess) e = cudaMemcpy(c->d_consts, consts, sizeof consts, cudaMemcpyHostToDevice);
@@ -474,7 +530,7 @@ cpb_status cpb_te_base_mul_batch_dev(cpb_te_base_ctx* c, const uint64_t* scalars
     if (!scalars || !out_xy) return fail(CPB_NULL_POINTER, "null array");
     CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
-    return base_mul_dev(c, (const u32*)scalars, 8, (u32*)out_xy, n, (cudaStream_t)stream);
+    return on_curve(c, [&](auto k) { return base_mul_dev<decltype(k)>(c, (const u32*)scalars, 8, (u32*)out_xy, n, (cudaStream_t)stream); });
     });
 }
 
@@ -486,8 +542,10 @@ cpb_status cpb_schnorr_sign_batch_dev(cpb_te_base_ctx* c, const uint8_t* salt, c
     if (!salt || !sks || !nonces || !msg_offsets || !sigs_out || !signed_out) return fail(CPB_NULL_POINTER, "null array");
     CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
-    return sign_dev(c, salt_of(salt), (const u32*)sks, (const u32*)nonces, msgs, (const u64*)msg_offsets, (u32*)sigs_out, signed_out, n,
-                    (cudaStream_t)stream);
+    return on_curve(c, [&](auto k) {
+        return sign_dev<decltype(k)>(c, salt_of(salt), (const u32*)sks, (const u32*)nonces, msgs, (const u64*)msg_offsets, (u32*)sigs_out,
+                                     signed_out, n, (cudaStream_t)stream);
+    });
     });
 }
 
@@ -499,7 +557,10 @@ cpb_status cpb_schnorr_verify_batch_dev(cpb_te_base_ctx* c, const uint8_t* salt,
     if (!salt || !pks_xy || !msg_offsets || !sigs || !ok_out) return fail(CPB_NULL_POINTER, "null array");
     CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
-    return verify_dev(c, salt_of(salt), (const u32*)pks_xy, msgs, (const u64*)msg_offsets, (const u32*)sigs, ok_out, n, (cudaStream_t)stream);
+    return on_curve(c, [&](auto k) {
+        return verify_dev<decltype(k)>(c, salt_of(salt), (const u32*)pks_xy, msgs, (const u64*)msg_offsets, (const u32*)sigs, ok_out, n,
+                                       (cudaStream_t)stream);
+    });
     });
 }
 
@@ -512,10 +573,9 @@ cpb_status cpb_schnorr_randomize_public_key_batch_dev(cpb_te_base_ctx* c, const 
     CPB_TRY(check_rand_len(len));
     CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
-    cudaStream_t st = (cudaStream_t)stream;
-    k_schnorr_rand_pk<<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, (const u32*)pks_xy, randomness, (long)len, (long)stride, (u32*)out_xy,
-                                                       (long)n, 0);
-    return launched("k_schnorr_rand_pk");
+    return on_curve(c, [&](auto k) {
+        return rand_pk_dev<decltype(k)>(c, (const u32*)pks_xy, randomness, len, stride, (u32*)out_xy, n, (cudaStream_t)stream);
+    });
     });
 }
 
@@ -527,10 +587,9 @@ cpb_status cpb_schnorr_randomize_signature_batch_dev(cpb_te_base_ctx* c, const u
     if (!sigs || !sigs_out || (len && !randomness)) return fail(CPB_NULL_POINTER, "null array");
     CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
-    cudaStream_t st = (cudaStream_t)stream;
-    k_schnorr_rand_sig<<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, (const u32*)sigs, randomness, (long)len, (long)stride, (u32*)sigs_out,
-                                                        (long)n, 0);
-    return launched("k_schnorr_rand_sig");
+    return on_curve(c, [&](auto k) {
+        return rand_sig_dev<decltype(k)>(c, (const u32*)sigs, randomness, len, stride, (u32*)sigs_out, n, (cudaStream_t)stream);
+    });
     });
 }
 
@@ -542,7 +601,9 @@ cpb_status cpb_elgamal_encrypt_batch_dev(cpb_te_base_ctx* c, const uint64_t* pks
     if (!pks_xy || !msgs_xy || !rands || !ciphertexts_out) return fail(CPB_NULL_POINTER, "null array");
     CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
-    return encrypt_dev(c, (const u32*)pks_xy, (const u32*)msgs_xy, (const u32*)rands, (u32*)ciphertexts_out, n, (cudaStream_t)stream);
+    return on_curve(c, [&](auto k) {
+        return encrypt_dev<decltype(k)>(c, (const u32*)pks_xy, (const u32*)msgs_xy, (const u32*)rands, (u32*)ciphertexts_out, n, (cudaStream_t)stream);
+    });
     });
 }
 
@@ -554,9 +615,9 @@ cpb_status cpb_elgamal_decrypt_batch_dev(cpb_te_base_ctx* c, const uint64_t* sks
     if (!sks || !ciphertexts || !msgs_out) return fail(CPB_NULL_POINTER, "null array");
     CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
-    cudaStream_t st = (cudaStream_t)stream;
-    k_elgamal_decrypt<<<grid_of(n), kSigBlock, 0, st>>>(c->d_consts, (const u32*)sks, (const u32*)ciphertexts, (u32*)msgs_out, (long)n, 0);
-    return launched("k_elgamal_decrypt");
+    return on_curve(c, [&](auto k) {
+        return decrypt_dev<decltype(k)>(c, (const u32*)sks, (const u32*)ciphertexts, (u32*)msgs_out, n, (cudaStream_t)stream);
+    });
     });
 }
 
@@ -587,7 +648,7 @@ cpb_status cpb_te_base_mul_batch(cpb_te_base_ctx* c, const uint64_t* scalars, ui
     u32 *d_s, *d_o;
     CPB_TRY(h.up(d_s, scalars, 32 * n));
     CPB_TRY(h.alloc(d_o, 64 * n));
-    CPB_TRY(base_mul_dev(c, d_s, 8, d_o, n, c->stream));
+    CPB_TRY(on_curve(c, [&](auto k) { return base_mul_dev<decltype(k)>(c, d_s, 8, d_o, n, c->stream); }));
     return h.down(out_xy, d_o, 64 * n);
     });
 }
@@ -613,7 +674,7 @@ cpb_status cpb_schnorr_sign_batch(cpb_te_base_ctx* c, const uint8_t* salt, const
     CPB_TRY(h.messages(d_m, d_off, msgs, msg_offsets, n));
     CPB_TRY(h.alloc(d_sig, 64 * n));
     CPB_TRY(h.alloc(d_ok, n));
-    CPB_TRY(sign_dev(c, salt_of(salt), d_sk, d_k, d_m, d_off, d_sig, d_ok, n, c->stream));
+    CPB_TRY(on_curve(c, [&](auto k) { return sign_dev<decltype(k)>(c, salt_of(salt), d_sk, d_k, d_m, d_off, d_sig, d_ok, n, c->stream); }));
     CPB_CUDA(cudaMemcpyAsync(signed_out, d_ok, n, cudaMemcpyDeviceToHost, c->stream));
     return h.down(sigs_out, d_sig, 64 * n);
     });
@@ -639,7 +700,7 @@ cpb_status cpb_schnorr_verify_batch(cpb_te_base_ctx* c, const uint8_t* salt, con
     CPB_TRY(h.up(d_sig, sigs, 64 * n));
     CPB_TRY(h.messages(d_m, d_off, msgs, msg_offsets, n));
     CPB_TRY(h.alloc(d_ok, n));
-    CPB_TRY(verify_dev(c, salt_of(salt), d_pk, d_m, d_off, d_sig, d_ok, n, c->stream));
+    CPB_TRY(on_curve(c, [&](auto k) { return verify_dev<decltype(k)>(c, salt_of(salt), d_pk, d_m, d_off, d_sig, d_ok, n, c->stream); }));
     return h.down(ok_out, d_ok, n);
     });
 }
@@ -704,7 +765,7 @@ cpb_status cpb_elgamal_encrypt_batch(cpb_te_base_ctx* c, const uint64_t* pks_xy,
     CPB_TRY(h.up(d_m, msgs_xy, 64 * n));
     CPB_TRY(h.up(d_r, rands, 32 * n));
     CPB_TRY(h.alloc(d_o, 128 * n));
-    CPB_TRY(encrypt_dev(c, d_pk, d_m, d_r, d_o, n, c->stream));
+    CPB_TRY(on_curve(c, [&](auto k) { return encrypt_dev<decltype(k)>(c, d_pk, d_m, d_r, d_o, n, c->stream); }));
     return h.down(ciphertexts_out, d_o, 128 * n);
     });
 }

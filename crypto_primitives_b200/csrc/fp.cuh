@@ -76,6 +76,20 @@ struct Bls12_377_Fr {
     CPB_FIELD_TABLE(ONE, 0xfffffff3u, 0x7d1c7fffu, 0x6ffffff2u, 0x7257f50fu, 0x512c0feeu, 0x16d81575u, 0x2bbb9a9du, 0x0d4bda32u)
     CPB_FIELD_TABLE(R2, 0xb861857bu, 0x25d577bau, 0x8860591fu, 0xcc2c27b5u, 0xe5dc8593u, 0xa7cc008fu, 0xeff1c939u, 0x011fdae7u)
 };
+// Scalar field of ed-on-BLS12-377 (the prime-order subgroup's order r, 251 bits).  Signatures and encryption only: no
+// Poseidon kernel is instantiated for it, so it carries none of the Poseidon knobs above.
+struct Ed_On_Bls12_377_Fr {
+    static constexpr bool LAZY5 = false;
+    static constexpr int P0_POW = 0;          // k > 0: p[0] == 2^32 - 2^k + 1
+    static constexpr bool P0_ONE = false;       // p[0] == 1  (then -p^-1 mod 2^32 == -1)
+    static constexpr bool P1_ALLONES = false;   // p[1] == 0xffffffff
+    static constexpr int ID = 4;
+    static constexpr u32 NINV = 0x70e3da01u;
+    static constexpr int BITS = 251;
+    CPB_FIELD_TABLE(P, 0xc33fd9ffu, 0xb95aee9au, 0xc43c8afeu, 0x5293a3afu, 0x970dec00u, 0x982d1347u, 0xa68b2955u, 0x04aad957u)
+    CPB_FIELD_TABLE(ONE, 0xd0880436u, 0xe6d1ab5au, 0x9b3aae44u, 0x94db78ecu, 0x231037eeu, 0xe67deee6u, 0xdea547f1u, 0x03f62782u)
+    CPB_FIELD_TABLE(R2, 0x6a55d45eu, 0x375699cdu, 0x7a73da73u, 0xf639c3f5u, 0xcd027a21u, 0xca06049cu, 0xef02d841u, 0x047ada1eu)
+};
 
 // ---------------------------------------------------------------------------------------
 // Element-wise helpers (all loops fully unrolled: limbs live in registers).

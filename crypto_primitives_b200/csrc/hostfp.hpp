@@ -166,17 +166,23 @@ private:
     }
 };
 
-// Known moduli, indexed by the C-ABI field id (include/cpb200.h).
-inline const u64* field_modulus(int field_id) {
-    static const u64 M[4][4] = {
+// Every field with device arithmetic, indexed by the C-ABI field id (include/cpb200.h).  The field-level entry points
+// (modulus, Montgomery conversion, element serialisation) accept all of them.
+inline const u64* element_field_modulus(int field_id) {
+    static const u64 M[5][4] = {
         {0xffffffff00000001ull, 0x53bda402fffe5bfeull, 0x3339d80809a1d805ull, 0x73eda753299d7d48ull},  // BLS12-381 Fr
         {0x43e1f593f0000001ull, 0x2833e84879b97091ull, 0xb85045b68181585dull, 0x30644e72e131a029ull},  // BN254 Fr
         {0xd0970e5ed6f72cb7ull, 0xa6682093ccc81082ull, 0x06673b0101343b00ull, 0x0e7db4ea6533afa9ull},  // Jubjub Fr
         {0x0a11800000000001ull, 0x59aa76fed0000001ull, 0x60b44d1e5c37b001ull, 0x12ab655e9a2ca556ull},  // BLS12-377 Fr
+        {0xb95aee9ac33fd9ffull, 0x5293a3afc43c8afeull, 0x982d1347970dec00ull, 0x04aad957a68b2955ull},  // ed-on-BLS12-377 Fr
     };
-    if (field_id < 0 || field_id > 3) return nullptr;
+    if (field_id < 0 || field_id > 4) return nullptr;
     return M[field_id];
 }
+
+// The hash fields (ids 0..3): the fields of Poseidon parameters, contexts and Merkle digests.  Every entry point that
+// builds or reads hashes validates its field id here, so the scalar field of ed-on-BLS12-377 stays unknown to them.
+inline const u64* field_modulus(int field_id) { return field_id <= 3 ? element_field_modulus(field_id) : nullptr; }
 
 typedef std::vector<Fe> FeVec;
 

@@ -5,7 +5,7 @@ from __future__ import annotations
 
 from dataclasses import dataclass
 
-from .fields import BLS12_377_FR, BLS12_381_FR, Field
+from .fields import BLS12_377_FR, BLS12_381_FR, ED_ON_BLS12_377_FR, JUBJUB_FR, Field
 
 
 @dataclass(frozen=True)
@@ -17,6 +17,7 @@ class TECurve:
     cofactor: int
     d_num: int
     d_den: int          # d = -(d_num/d_den) when d_den != 1 else d_num ; a = -1
+    scalar_field: Field     # the field of scalar_modulus: secret keys, nonces and signatures are its elements
 
     @property
     def q(self) -> int:
@@ -99,7 +100,8 @@ class TECurve:
 
 
 JUBJUB = TECurve(0, "jubjub", BLS12_381_FR, 0x0E7DB4EA6533AFA906673B0101343B00A6682093CCC81082D0970E5ED6F72CB7,
-                 8, 10240, 10241)
+                 8, 10240, 10241, JUBJUB_FR)
 ED_ON_BLS12_377 = TECurve(1, "ed_on_bls12_377", BLS12_377_FR,
-                          0x04AAD957A68B2955982D1347970DEC005293A3AFC43C8AFEB95AEE9AC33FD9FF, 4, 3021, 1)
+                          0x04AAD957A68B2955982D1347970DEC005293A3AFC43C8AFEB95AEE9AC33FD9FF, 4, 3021, 1,
+                          ED_ON_BLS12_377_FR)
 CURVES = {c.name: c for c in (JUBJUB, ED_ON_BLS12_377)}

@@ -1,7 +1,7 @@
 """encryption::elgamal::{Parameters, ElGamal} -- host mirror of R/encryption/elgamal/mod.rs over the CUDA library, for
-ElGamal<EdwardsProjective (Jubjub)> (the reference's test curve, mod.rs:102-128).
+ElGamal<EdwardsProjective> over Jubjub (the reference's test curve, mod.rs:102-128) or ed-on-BLS12-377 (`Parameters.curve`).
 
-Layouts as in signature/schnorr.py: scalars (..., 4) Fr Montgomery limbs, points (..., 2, 4) affine Montgomery limbs, a
+Layouts as in signature/schnorr.py: scalars (..., 4) Montgomery limbs of the curve's scalar field, points (..., 2, 4) affine Montgomery limbs, a
 ciphertext (c1, c2) is (..., 2, 2, 4).  The `*_dev` forms take torch CUDA int64 tensors on the current stream."""
 from __future__ import annotations
 
@@ -9,7 +9,6 @@ import numpy as np
 
 from .. import _native as N
 from ..curves import JUBJUB, TECurve
-from ..fields import JUBJUB_FR
 from ..signature.schnorr import BaseParameters, _points, _scalars, _torch_stream, _u64, base_mul_batch
 
 
@@ -29,7 +28,7 @@ class ElGamal:
     @staticmethod
     def keygen(parameters: Parameters, rng, device: int = 0):
         """mod.rs:55-67 -> (public_key (2, 4), secret_key (4,))."""
-        sk = JUBJUB_FR.elements([rng.field(parameters.curve.scalar_modulus)])
+        sk = parameters.curve.scalar_field.elements([rng.field(parameters.curve.scalar_modulus)])
         return base_mul_batch(parameters, sk, device)[0], sk[0]
 
     @staticmethod

@@ -70,4 +70,6 @@ BLS12_381_FR = Field(0, "bls12_381_fr")
 BN254_FR = Field(1, "bn254_fr")
 JUBJUB_FR = Field(2, "jubjub_fr")
 BLS12_377_FR = Field(3, "bls12_377_fr")
-FIELDS = {f.name: f for f in (BLS12_381_FR, BN254_FR, JUBJUB_FR, BLS12_377_FR)}
+FIELDS = {f.name: f for f in (BLS12_381_FR, BN254_FR, JUBJUB_FR, BLS12_377_FR)}     # the hash fields (Poseidon, Merkle)
+# The scalar field of ed-on-BLS12-377: the field-level calls above and the signature layer only, so not in FIELDS.
+ED_ON_BLS12_377_FR = Field(4, "ed_on_bls12_377_fr")

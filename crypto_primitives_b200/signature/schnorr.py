@@ -1,8 +1,9 @@
 """signature::schnorr::{Parameters, Schnorr} -- host mirror of R/signature/schnorr/mod.rs over the CUDA library, for
-Schnorr<EdwardsProjective (Jubjub), Blake2s256>, the instantiation of the reference's tests (R/signature/mod.rs:52-105).
+Schnorr<EdwardsProjective, Blake2s256> over Jubjub, the instantiation of the reference's tests (R/signature/mod.rs:52-105), and
+over ed-on-BLS12-377, the curve of the reference's signature benchmark (R/benches/signature.rs:5-10); `Parameters.curve` picks it.
 
-Scalars (secret keys, nonces, s and e) are Fr elements as Montgomery limbs, numpy uint64 (..., 4) (`cp.JUBJUB_FR.elements`
-converts Python ints); points are affine Montgomery limbs (..., 2, 4); a signature is (prover_response, verifier_challenge),
+Scalars (secret keys, nonces, s and e) are elements of the curve's scalar field as Montgomery limbs, numpy uint64 (..., 4)
+(`parameters.curve.scalar_field.elements` converts Python ints); points are affine Montgomery limbs (..., 2, 4); a signature is (prover_response, verifier_challenge),
 (..., 2, 4).  The single-item functions keep the trait signatures; the `*_batch` forms are the GPU path.  The `*_dev` forms take
 torch CUDA tensors (int64 views of the same layouts) and run asynchronously on the current torch stream.
 Signing is not constant time: secret scalars select table entries by value, as the reference's `mul` does.
@@ -17,7 +18,6 @@ import numpy as np
 
 from .. import _native as N
 from ..curves import JUBJUB, TECurve
-from ..fields import JUBJUB_FR
 
 
 def _u8(a):
@@ -64,7 +64,7 @@ class BaseParameters:
             h = _CONTEXTS.get(key)
             if h is None:
                 out = N.vp()
-                N.check(N.lib.cpb_te_base_ctx_create(self.curve.id, _u64(self.generator), device, C.byref(out)))
+                N.check(N.lib.cpb_te_base_ctx_create_ex(self.curve.id, _u64(self.generator), device, C.byref(out)))
                 h = _Ctx(out.value)
                 _CONTEXTS[key] = h
             self._ctx[device] = h
@@ -133,7 +133,7 @@ def _torch_stream():
 
 
 class Schnorr:
-    """SignatureScheme for Schnorr<Jubjub, Blake2s256> (mod.rs:40-183)."""
+    """SignatureScheme for Schnorr<C, Blake2s256> (mod.rs:40-183), C = Jubjub or ed-on-BLS12-377."""
 
     @staticmethod
     def setup(rng, curve: TECurve = JUBJUB) -> Parameters:
@@ -145,7 +145,7 @@ class Schnorr:
     @staticmethod
     def keygen(parameters: Parameters, rng, device: int = 0):
         """mod.rs:65-78 -> (public_key (2, 4), secret_key (4,))."""
-        sk = JUBJUB_FR.elements([rng.field(parameters.curve.scalar_modulus)])
+        sk = parameters.curve.scalar_field.elements([rng.field(parameters.curve.scalar_modulus)])
         return Schnorr.keygen_batch(parameters, sk, device)[0], sk[0]
 
     @staticmethod
@@ -169,7 +169,7 @@ class Schnorr:
         todo = np.arange(n)
         r = parameters.curve.scalar_modulus
         while todo.size:
-            nonces = JUBJUB_FR.elements([rng.field(r) for _ in range(todo.size)])
+            nonces = parameters.curve.scalar_field.elements([rng.field(r) for _ in range(todo.size)])
             s, ok = Schnorr.sign_with_nonces_batch(parameters, sks[todo], nonces, [msgs[i] for i in todo], device)
             sigs[todo[ok]] = s[ok]
             todo = todo[~ok]

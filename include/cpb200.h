@@ -59,7 +59,11 @@ typedef enum cpb_field {
     CPB_BLS12_381_FR = 0, /* the reference's test field, R/sponge/test.rs:5-12 */
     CPB_BN254_FR = 1,
     CPB_JUBJUB_FR = 2,    /* ark_ed_on_bls12_381::Fr, R/merkle_tree/tests/mod.rs:195 */
-    CPB_BLS12_377_FR = 3  /* R/crh/poseidon/constraints.rs:133-190 */
+    CPB_BLS12_377_FR = 3, /* R/crh/poseidon/constraints.rs:133-190 */
+    CPB_ED_ON_BLS12_377_FR = 4  /* ark_ed_on_bls12_377::Fr, the scalar field of CPB_ED_ON_BLS12_377 (R/benches/signature.rs:5-10).  Known
+                                   to the field-level calls only (cpb_field_modulus, cpb_field_{to,from}_montgomery[_dev],
+                                   cpb_field_serialized_size, cpb_field_{serialize,deserialize}); every call that takes the field of a hash
+                                   (Poseidon, Merkle, path wire formats) answers CPB_BAD_PARAMS for it, as for an unknown id. */
 } cpb_field;
 
 typedef enum cpb_curve {
@@ -78,8 +82,10 @@ const char* cpb_last_error(void);
 
 /* ABI revision of this header: bumped when entry points or status codes are added (2 = CPB_INTERNAL_ERROR, cpb_abi_version; 3 = _dev field conversion, host pinning, launch count, multi-GPU build, CPB_NCCL_ERROR, wire formats; 4 = ragged Poseidon batches: CRH, sponge, Merkle build and path verification over inputs of different lengths; 5 = Merkle update and
  * check_update of Poseidon-node trees, in place on device arrays or over host arrays; later additions under 5 are additive: Merkle path verification of the Pedersen
- * trees, batched duplex sponges with the cpb_sponge_mode type, ragged duplex calls with a mode per sponge -- a library that has
- * them exports cpb_poseidon_duplex_absorb_ragged). */
+ * trees, batched duplex sponges with the cpb_sponge_mode type, ragged duplex calls with a mode per sponge (a library that has
+ * them exports cpb_poseidon_duplex_absorb_ragged), the field CPB_ED_ON_BLS12_377_FR with signatures and encryption over
+ * CPB_ED_ON_BLS12_377 (a library that has them exports cpb_te_base_ctx_create_ex and answers CPB_OK to
+ * cpb_field_modulus(CPB_ED_ON_BLS12_377_FR, ...)). */
 #define CPB_ABI_VERSION 5
 int cpb_abi_version(void);
 int cpb_version(void);
@@ -582,11 +588,14 @@ cpb_status cpb_multipath_deserialize(int leaf_kind, int leaf_id, int inner_kind,
                                      uint64_t* suffix_lengths, uint64_t* suffixes, uint64_t* leaf_indexes, size_t cap_paths,
                                      size_t cap_suffix_digests);
 
-/* ---- Schnorr signatures, ElGamal encryption and the Blake2s commitment over Jubjub ------------------------------------ */
+/* ---- Schnorr signatures, ElGamal encryption and the Blake2s commitment over Jubjub and ed-on-BLS12-377 ---------------- */
 /* signature::schnorr::Schnorr<EdwardsProjective, Blake2s256> (R/signature/schnorr/mod.rs) and encryption::elgamal::ElGamal
  * (R/encryption/elgamal/mod.rs) for C = ark_ed_on_bls12_381 (Jubjub), the curve of both reference test suites
- * (R/signature/mod.rs:52-105, R/encryption/elgamal/mod.rs:102-128); commitment::blake2s::Commitment (R/commitment/blake2s/mod.rs).
- * Layouts: a scalar is an Fr (Jubjub scalar field, CPB_JUBJUB_FR) element as Montgomery limbs, 4 x uint64; a point is affine
+ * (R/signature/mod.rs:52-105, R/encryption/elgamal/mod.rs:102-128), and for C = ark_ed_on_bls12_377, the curve of the reference's
+ * signature benchmark (R/benches/signature.rs:5-10); commitment::blake2s::Commitment (R/commitment/blake2s/mod.rs).  The curve is
+ * the context's (cpb_te_base_ctx_create_ex).
+ * Layouts: a scalar is an Fr element of the context's curve (CPB_JUBJUB_FR for Jubjub, CPB_ED_ON_BLS12_377_FR for
+ * ed-on-BLS12-377) as Montgomery limbs, 4 x uint64; a point is affine over the curve's base field
  * x || y, 8 x uint64; a signature is (prover_response s, verifier_challenge e), 8 x uint64; a ciphertext (c1, c2), 16 x uint64.
  * Messages are ragged bytes: message i = msgs[msg_offsets[i] .. msg_offsets[i+1]), msg_offsets has n + 1 uint64 (the rules of the
  * ragged Poseidon batches above: host forms reject decreasing offsets with CPB_BAD_LENGTH and copy only msgs[offsets[0] ..
@@ -598,19 +607,22 @@ cpb_status cpb_multipath_deserialize(int leaf_kind, int leaf_id, int inner_kind,
 typedef struct cpb_te_base_ctx cpb_te_base_ctx;
 /* Parameters{generator} of both schemes (schnorr/mod.rs:24-29 without the salt, elgamal/mod.rs:14-16), affine (x, y).  Builds the
  * fixed-base tables of the generator on the device: a Pedersen context (library default chunk width) whose 256 generators are
- * 2^k G, so s*G is the Pedersen hash of the 32-byte little-endian canonical scalar.  curve_id != CPB_JUBJUB -> CPB_UNSUPPORTED (no
- * device arithmetic in the scalar field of ed-on-BLS12-377); a generator that is not a reduced point on the curve -> CPB_BAD_PARAMS.
+ * 2^k G, so s*G is the Pedersen hash of the 32-byte little-endian canonical scalar.  cpb_te_base_ctx_create is the Jubjub form:
+ * curve_id != CPB_JUBJUB -> CPB_UNSUPPORTED, as it always was.  cpb_te_base_ctx_create_ex takes curve_id CPB_JUBJUB or
+ * CPB_ED_ON_BLS12_377 (any other id -> CPB_UNSUPPORTED) and is otherwise the same call; a library that exports it has signatures and
+ * encryption over ed-on-BLS12-377.  Both: a generator that is not a reduced point on the curve -> CPB_BAD_PARAMS.
  * Nothing else is assumed about it: it need not lie in the prime-order subgroup. */
 cpb_status cpb_te_base_ctx_create(int curve_id, const uint64_t* generator_xy, int device, cpb_te_base_ctx** out);
+cpb_status cpb_te_base_ctx_create_ex(int curve_id, const uint64_t* generator_xy, int device, cpb_te_base_ctx** out);
 void cpb_te_base_ctx_destroy(cpb_te_base_ctx* ctx);
 /* keygen of both schemes (schnorr/mod.rs:65-78, elgamal/mod.rs:55-67): out[i] = scalars[i] * G. */
 cpb_status cpb_te_base_mul_batch(cpb_te_base_ctx* ctx, const uint64_t* scalars, uint64_t* out_xy, size_t n);
 cpb_status cpb_te_base_mul_batch_dev(cpb_te_base_ctx* ctx, const uint64_t* scalars, uint64_t* out_xy, size_t n, void* stream);
 /* Schnorr::sign (schnorr/mod.rs:80-115), one loop iteration per item with the given nonce k: R = k*G, e =
  * Fr::from_random_bytes(Blake2s256(salt || compress(R) || u64_le(len) || msg)), s = k - e*sk.  salt: 32 bytes in HOST memory in both
- * forms (Parameters.salt), copied into the launch.  signed_out[i] = 0 when the challenge is not a field element (about 9.4 % of
- * nonces: the digest keeps its low 252 bits and must be below r); the caller draws a new nonce for that item, as the reference's
- * loop does.  sigs_out[i] is then (0, 0). */
+ * forms (Parameters.salt), copied into the launch.  signed_out[i] = 0 when the challenge is not a field element: the digest
+ * keeps its low MODULUS_BIT_SIZE bits and must be below r, which fails for about 1 - r / 2^bits of nonces (Jubjub: 252 bits,
+ * 9.4 %; ed-on-BLS12-377: 251 bits, 41.7 %); the caller draws a new nonce for that item, as the reference's loop does.  sigs_out[i] is then (0, 0). */
 cpb_status cpb_schnorr_sign_batch(cpb_te_base_ctx* ctx, const uint8_t* salt, const uint64_t* sks, const uint64_t* nonces, const uint8_t* msgs,
                                   const uint64_t* msg_offsets, uint64_t* sigs_out, uint8_t* signed_out, size_t n);
 cpb_status cpb_schnorr_sign_batch_dev(cpb_te_base_ctx* ctx, const uint8_t* salt, const uint64_t* sks, const uint64_t* nonces, const uint8_t* msgs,

@@ -369,13 +369,14 @@ inline void ragged_pack(const std::vector<std::vector<uint8_t>>& inputs, std::ve
     values.push_back(0);                                  // never empty, so data() is a valid pointer
 }
 
-// Parameters{generator} shared by Schnorr and ElGamal over Jubjub, with the generator's fixed-base tables on the device.
+// Parameters{generator} shared by Schnorr and ElGamal, with the generator's fixed-base tables on the device.  curve:
+// CPB_JUBJUB or CPB_ED_ON_BLS12_377; scalars are then elements of CPB_JUBJUB_FR or CPB_ED_ON_BLS12_377_FR.
 class TeBase {
 public:
     Affine generator;
     explicit TeBase(const Affine& g, int curve = CPB_JUBJUB, int device = 0) : generator(g) {
         cpb_te_base_ctx* c = nullptr;
-        check(cpb_te_base_ctx_create(curve, g.x.data(), device, &c));
+        check(cpb_te_base_ctx_create_ex(curve, g.x.data(), device, &c));
         ctx_.reset(c, cpb_te_base_ctx_destroy);
     }
     cpb_te_base_ctx* ctx() const { return ctx_.get(); }
@@ -390,7 +391,7 @@ private:
     std::shared_ptr<cpb_te_base_ctx> ctx_;
 };
 
-namespace schnorr {   // Schnorr<Jubjub, Blake2s256>, R/signature/schnorr/mod.rs; SignatureScheme, R/signature/mod.rs:14-50
+namespace schnorr {   // Schnorr<C, Blake2s256>, R/signature/schnorr/mod.rs; SignatureScheme, R/signature/mod.rs:14-50
 
 struct Signature { Fe prover_response, verifier_challenge; };
 
@@ -399,6 +400,8 @@ struct Parameters {
     TeBase base;
     std::array<uint8_t, 32> salt;
     Parameters(const Affine& generator, const std::array<uint8_t, 32>& salt_, int device = 0) : base(generator, CPB_JUBJUB, device), salt(salt_) {}
+    Parameters(const Affine& generator, const std::array<uint8_t, 32>& salt_, cpb_curve curve, int device = 0)
+        : base(generator, curve, device), salt(salt_) {}
 };
 
 struct Schnorr {
@@ -453,10 +456,10 @@ struct Schnorr {
 
 }  // namespace schnorr
 
-namespace elgamal {   // ElGamal<Jubjub>, R/encryption/elgamal/mod.rs; AsymmetricEncryptionScheme
+namespace elgamal {   // ElGamal<C>, R/encryption/elgamal/mod.rs; AsymmetricEncryptionScheme
 
 struct Ciphertext { Affine c1, c2; };
-using Parameters = TeBase;   // elgamal::Parameters{generator} (mod.rs:14-16)
+using Parameters = TeBase;   // elgamal::Parameters{generator} (mod.rs:14-16); TeBase(generator, curve, device)
 
 struct ElGamal {
     // mod.rs:69-84

@@ -1,9 +1,11 @@
 """Throughput of the Schnorr / ElGamal / Blake2s-commitment kernels (include/cpb200.h) on one GPU: keygen, sign, verify, ElGamal
 encrypt and decrypt, and the Blake2s commitment, at n = 2^20 items with messages of 32..256 bytes, through the _dev forms on
 device-resident inputs.  CUDA events around each call, median of repeated calls after a warm-up; the card name and power
-limit are read in the same run.  Writes profiles/h100_signature_perf.json (or --out).
+limit are read in the same run.  --curve picks the curve (default jubjub); ed_on_bls12_377 also times sign and verify on the
+reference benchmark's message, [100u8; 128] for every item (R/benches/signature.rs).  Writes
+profiles/h100_signature_perf.json for Jubjub, profiles/h100_signature_ed377_perf.json for ed-on-BLS12-377 (or --out).
 
-    python tools/perf_signature.py [--n 1048576] [--reps 5] [--out profiles/h100_signature_perf.json]
+    python tools/perf_signature.py [--curve jubjub|ed_on_bls12_377] [--n 1048576] [--reps 5] [--out FILE]
 """
 from __future__ import annotations
 
@@ -50,18 +52,22 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, default=1 << 20)
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_signature_perf.json"))
+    ap.add_argument("--curve", choices=sorted(cp.curves.CURVES), default="jubjub")
+    ap.add_argument("--out", default=None)
     args = ap.parse_args()
+    curve = cp.curves.CURVES[args.curve]
+    if args.out is None:
+        args.out = os.path.join(ROOT, "profiles", "h100_signature_perf.json" if curve is cp.curves.JUBJUB else "h100_signature_ed377_perf.json")
     n = args.n
     dev = torch.device("cuda", 0)
     rng = OF.SplitMix64(1)
-    prm = Schnorr.setup(rng)
-    eprm = cp.encryption_elgamal.Parameters(prm.generator)
+    prm = Schnorr.setup(rng, curve)
+    eprm = cp.encryption_elgamal.Parameters(prm.generator, curve)
     g = np.random.default_rng(2)
-    r = cp.curves.JUBJUB.scalar_modulus
+    r = curve.scalar_modulus
     pyr = random.Random(3)
     # distinct random scalars for a slice, tiled: the kernels' work does not depend on the values beyond their bits
-    base = cp.JUBJUB_FR.elements([pyr.randrange(r) for _ in range(4096)])
+    base = curve.scalar_field.elements([pyr.randrange(r) for _ in range(4096)])
     sks = np.ascontiguousarray(np.tile(base, (n // 4096 + 1, 1))[:n])
     ks = np.ascontiguousarray(np.roll(sks, 1, axis=0))
     lens = g.integers(32, 257, n)
@@ -96,12 +102,26 @@ def main():
         "elgamal_decrypt": lambda: ElGamal.decrypt_dev(eprm, d_sk, d_ct, out=d_m),
         "blake2s_commit": lambda: Commitment.commit_dev(d_vals, d_off, d_rnd, out=d_cm),
     }
+    if curve is not cp.curves.JUBJUB:
+        # the reference benchmark's message for every item: sign, then verify what was signed
+        d_vals128 = t(np.full(128 * n, 100, dtype=np.uint8), torch.uint8)
+        d_off128 = t(np.arange(n + 1, dtype=np.uint64) * 128)
+        d_sig128, d_ok128 = Schnorr.sign_with_nonces_dev(prm, d_sk, d_k, d_vals128, d_off128)
+        d_vok128 = Schnorr.verify_dev(prm, d_pk, d_vals128, d_off128, d_sig128)
+        torch.cuda.synchronize()
+        signed128 = d_ok128.cpu().numpy().astype(bool)
+        checks["signed_fraction_128"] = float(signed128.mean())
+        checks["every_signed_item_verifies_128"] = bool(d_vok128.cpu().numpy().astype(bool)[signed128].all())
+        ops["sign_msg128"] = lambda: Schnorr.sign_with_nonces_dev(prm, d_sk, d_k, d_vals128, d_off128, sigs_out=d_sig128, signed_out=d_ok128)
+        ops["verify_msg128"] = lambda: Schnorr.verify_dev(prm, d_pk, d_vals128, d_off128, d_sig128, ok_out=d_vok128)
     results = {}
     for name, fn in ops.items():
         med, times = timed(fn, args.reps)
         results[name] = {"median_ms": med, "items_per_s": n / (med / 1e3), "times_ms": times}
         print(f"{name:16s} {med:9.2f} ms  {n / (med / 1e3) / 1e6:8.3f} M items/s", flush=True)
     out = {"gpu": gpu_info(), "n": n, "message_bytes": "uniform 32..256", "reps": args.reps, "checks": checks, "results": results}
+    if curve is not cp.curves.JUBJUB:
+        out = {"curve": curve.name, **out, "msg128": "[100u8; 128] for every item (sign_msg128, verify_msg128)"}
     os.makedirs(os.path.dirname(args.out), exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(out, f, indent=1)
