@@ -72,10 +72,16 @@ cpb_status check_device_arch(int device);
 // every synchronisation, which makes the next cudaMallocAsync re-map (and serialise) each time: keep it cached in the pool.
 void keep_pool_memory(int device);
 
-// Grow-only device scratch buffer owned by a context (guarded by the context mutex).
+inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// Grow-only device scratch buffer: one per context (guarded by the context mutex), or a local one freed on scope exit.
 struct Scratch {
     void* ptr = nullptr;
     size_t cap = 0;
+    Scratch() = default;
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    ~Scratch() { release(); }
     cpb_status reserve(size_t bytes) {
         if (bytes <= cap) return CPB_OK;
         if (ptr) cudaFree(ptr);
@@ -91,6 +97,64 @@ struct Scratch {
         ptr = nullptr;
         cap = 0;
     }
+};
+
+// How a host-pointer entry point stages its arrays through a Scratch arena on one stream.  Declare every region first (in: copied
+// up, out: copied back, inout: both, dev: device only; each call returns the region's offset), then upload() reserves the
+// 256-byte-aligned regions once and queues the uploads, at<T>(offset) gives the device pointers, and download() queues the copies
+// back and synchronises.  The destructor synchronises too, so no return path, errors included, leaves a copy from or to a caller's
+// buffer queued once the call (and the context mutex) is left.  A zero-byte region gets its own pointer and no copy.
+class HostStage {
+  public:
+    HostStage(Scratch& arena, cudaStream_t st) : arena_(arena), st_(st) {}
+    HostStage(const HostStage&) = delete;
+    HostStage& operator=(const HostStage&) = delete;
+    ~HostStage() {
+        if (!synced_) cudaStreamSynchronize(st_);
+    }
+    size_t in(const void* h, size_t bytes) { return add(const_cast<void*>(h), bytes, kIn); }
+    size_t out(void* h, size_t bytes) { return add(h, bytes, kOut); }
+    size_t inout(void* h, size_t bytes) { return add(h, bytes, kIn | kOut); }
+    size_t dev(size_t bytes) { return add(nullptr, bytes, 0); }
+    template <class T> T* at(size_t off) const { return (T*)((char*)arena_.ptr + off); }
+
+    cpb_status upload() {
+        if (n_ > kMax) return fail(CPB_INTERNAL_ERROR, "more than %d staged regions", kMax);
+        CPB_TRY(arena_.reserve(total_));
+        for (int i = 0; i < n_; i++)
+            if ((r_[i].dir & kIn) && r_[i].bytes)
+                CPB_CUDA(cudaMemcpyAsync(at<char>(r_[i].off), r_[i].host, r_[i].bytes, cudaMemcpyHostToDevice, st_));
+        return CPB_OK;
+    }
+    cpb_status download() {
+        for (int i = 0; i < n_; i++)
+            if ((r_[i].dir & kOut) && r_[i].bytes)
+                CPB_CUDA(cudaMemcpyAsync(r_[i].host, at<char>(r_[i].off), r_[i].bytes, cudaMemcpyDeviceToHost, st_));
+        synced_ = true;
+        CPB_CUDA(cudaStreamSynchronize(st_));
+        return CPB_OK;
+    }
+
+  private:
+    enum { kIn = 1, kOut = 2, kMax = 10 };
+    struct Region {
+        void* host;
+        size_t bytes, off;
+        int dir;
+    };
+    size_t add(void* h, size_t bytes, int dir) {
+        const size_t off = total_;
+        total_ += align256(bytes ? bytes : 1);
+        if (n_ < kMax) r_[n_] = Region{h, bytes, off, dir};
+        n_++;
+        return off;
+    }
+    Scratch& arena_;
+    cudaStream_t st_;
+    Region r_[kMax];
+    int n_ = 0;
+    size_t total_ = 0;
+    bool synced_ = false;
 };
 
 #if defined(__CUDACC__)

@@ -201,7 +201,7 @@ cpb_status update_digests_dev(cpb_pedersen_ctx* node, u32* leaf_nodes, u32* node
     }
     const int lt = warp_start_level(X.h, k);
     const size_t n_arr = lt >= 0 ? (size_t)X.off[lt] : 0;      // arrival counters of the levels above the warp launch's start
-    const size_t rows_b = upd_up(128 * (size_t)upd_width(X.h - 1, k));   // the widest inner level's rows
+    const size_t rows_b = align256(128 * (size_t)upd_width(X.h - 1, k));   // the widest inner level's rows
     const size_t row_len = two_to_one_len(node);
     UpdBuffers B;
     CPB_TRY(upd_layout(X, n, k, rows_b + 4 * n_arr + 4, kPedW, st, B));

@@ -145,7 +145,7 @@ cpb_status check_mixed_ctxs(cpb_pedersen_ctx* leaf, cpb_poseidon_ctx* node, size
     return check_len(leaf, leaf_len, false);
 }
 
-// Host forms: the proofs go up on the leaf context's stream under its mutex, the device code runs there, ok comes back.  `dw`: words of
+// Host forms: the proofs go up through the leaf context's arena, on its stream under its mutex, the device code runs there, ok comes back.  `dw`: words of
 // one digest (16: affine point, 8: field element).
 template <class Dev>
 cpb_status verify_host(cpb_pedersen_ctx* leaf, size_t dw, const uint64_t* root, const uint8_t* leaves, size_t leaf_len,
@@ -153,25 +153,14 @@ cpb_status verify_host(cpb_pedersen_ctx* leaf, size_t dw, const uint64_t* root, 
                        Dev&& dev) {
     std::lock_guard<std::mutex> lk(leaf->mu);
     DeviceGuard g(leaf->device);
+    HostStage S(leaf->arena, leaf->stream);
     const size_t db = 4 * dw;
-    const size_t b_root = db, b_leaves = n * leaf_len, b_sib = n * db, b_path = n * path_len * db, b_idx = n * 8;
-    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t o_leaves = up(b_root), o_sib = o_leaves + up(b_leaves), o_path = o_sib + up(b_sib), o_idx = o_path + up(b_path),
-                 total = o_idx + up(b_idx);
-    CPB_TRY(leaf->s_in.reserve(total));
-    CPB_TRY(leaf->s_out.reserve(n));
-    char* d = (char*)leaf->s_in.ptr;
-    cudaStream_t st = leaf->stream;
-    CPB_CUDA(cudaMemcpyAsync(d, root, b_root, cudaMemcpyHostToDevice, st));
-    if (b_leaves) CPB_CUDA(cudaMemcpyAsync(d + o_leaves, leaves, b_leaves, cudaMemcpyHostToDevice, st));
-    CPB_CUDA(cudaMemcpyAsync(d + o_sib, leaf_sibs, b_sib, cudaMemcpyHostToDevice, st));
-    if (b_path) CPB_CUDA(cudaMemcpyAsync(d + o_path, paths, b_path, cudaMemcpyHostToDevice, st));
-    CPB_CUDA(cudaMemcpyAsync(d + o_idx, indexes, b_idx, cudaMemcpyHostToDevice, st));
-    CPB_TRY(dev((const u32*)d, (const uint8_t*)(d + o_leaves), (const u32*)(d + o_sib), (const u32*)(d + o_path),
-                (const unsigned long long*)(d + o_idx), (unsigned char*)leaf->s_out.ptr, st));
-    CPB_CUDA(cudaMemcpyAsync(ok, leaf->s_out.ptr, n, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    const size_t o_root = S.in(root, db), o_leaves = S.in(leaves, n * leaf_len), o_sib = S.in(leaf_sibs, n * db),
+                 o_path = S.in(paths, n * path_len * db), o_idx = S.in(indexes, n * 8), o_ok = S.out(ok, n);
+    CPB_TRY(S.upload());
+    CPB_TRY(dev(S.at<u32>(o_root), S.at<uint8_t>(o_leaves), S.at<u32>(o_sib), S.at<u32>(o_path), S.at<unsigned long long>(o_idx),
+                S.at<unsigned char>(o_ok), leaf->stream));
+    return S.download();
 }
 
 }  // namespace

@@ -255,24 +255,20 @@ cpb_status cpb_merkle_poseidon_build_sharded(cpb_poseidon_ctx* leaf, cpb_poseido
     if ((!leaves && leaf_len) || !leaf_nodes || !non_leaf_nodes || (ex->world > 1 && !top_nodes)) return fail(CPB_NULL_POINTER, "null buffer");
     std::lock_guard<std::mutex> lk(leaf->mu);
     DeviceGuard g(leaf->device);
-    size_t in_b = n_local * leaf_len * 32, top_b = (size_t)(ex->world - 1) * 32;
-    CPB_TRY(leaf->s_in.reserve(in_b ? in_b : 32));
-    CPB_TRY(leaf->s_out.reserve(n_local * 32));
-    CPB_TRY(leaf->s_aux.reserve((n_local - 1) * 32 + top_b + 32));
     cudaStream_t st = leaf->stream;
-    u32* d_nodes = (u32*)leaf->s_aux.ptr;
-    u32* d_top = d_nodes + 8 * (n_local - 1);
+    HostStage S(leaf->arena, st);        // the leaves and levels move through MerkleHost; only the replicated top comes back here
+    const size_t o_in = S.dev(n_local * leaf_len * 32), o_leaf = S.dev(n_local * 32), o_nodes = S.dev((n_local - 1) * 32),
+                 o_top = S.out(top_nodes, (size_t)(ex->world - 1) * 32);
+    CPB_TRY(S.upload());
     MerkleHost H;
     H.leaves = (const u32*)leaves; H.leaf_nodes = (u32*)leaf_nodes; H.nodes = (u32*)non_leaf_nodes;
     if (ex->world == 1) {
-        CPB_TRY(merkle_build_streams(leaf, node, (const u32*)leaf->s_in.ptr, leaf_len, n_local, (u32*)leaf->s_out.ptr, d_nodes, st, &H));
+        CPB_TRY(merkle_build_streams(leaf, node, S.at<u32>(o_in), leaf_len, n_local, S.at<u32>(o_leaf), S.at<u32>(o_nodes), st, &H));
     } else {
-        ExchangeDev X = ex->next(d_top);
-        CPB_TRY(merkle_build_streams(leaf, node, (const u32*)leaf->s_in.ptr, leaf_len, n_local, (u32*)leaf->s_out.ptr, d_nodes, st, &H, &X));
-        CPB_CUDA(cudaMemcpyAsync(top_nodes, d_top, top_b, cudaMemcpyDeviceToHost, st));
+        ExchangeDev X = ex->next(S.at<u32>(o_top));
+        CPB_TRY(merkle_build_streams(leaf, node, S.at<u32>(o_in), leaf_len, n_local, S.at<u32>(o_leaf), S.at<u32>(o_nodes), st, &H, &X));
     }
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    return S.download();
     });
 }
 
@@ -380,16 +376,16 @@ cpb_status cpb_merkle_poseidon_build_multi(cpb_multi* m, cpb_poseidon_ctx* const
         cpb_poseidon_ctx* L = leaf_ctxs[d];
         std::lock_guard<std::mutex> lkd(L->mu);
         DeviceGuard gd(m->devices[d]);
-        CPB_TRY(L->s_in.reserve(per * leaf_len * 32 ? per * leaf_len * 32 : 32));
-        CPB_TRY(L->s_out.reserve(per * 32));
-        CPB_TRY(L->s_aux.reserve((per - 1) * 32));
+        HostStage S(L->arena, L->stream);
+        const size_t o_in = S.dev(per * leaf_len * 32), o_leaf = S.dev(per * 32), o_nodes = S.dev((per - 1) * 32);
+        CPB_TRY(S.upload());
         MerkleHost H;
         H.leaves = (const u32*)leaves + 8 * leaf_len * (per * d);
         H.leaf_nodes = (u32*)leaf_nodes + 8 * (per * d);
         H.nodes = (u32*)non_leaf_nodes;
         H.g = g; H.rank = (size_t)d;
-        const u32* d_leaves = (const u32*)L->s_in.ptr;
-        u32 *d_ln = (u32*)L->s_out.ptr, *d_nodes = (u32*)L->s_aux.ptr;
+        const u32* d_leaves = S.at<u32>(o_in);
+        u32 *d_ln = S.at<u32>(o_leaf), *d_nodes = S.at<u32>(o_nodes);
         if (G == 1 || m->use_nccl) {
             CPB_TRY(merkle_build_streams(L, node_ctxs[d], d_leaves, leaf_len, per, d_ln, d_nodes, L->stream, &H));
         } else {
@@ -402,8 +398,7 @@ cpb_status cpb_merkle_poseidon_build_multi(cpb_multi* m, cpb_poseidon_ctx* const
             CPB_TRY(merkle_build_streams(node_ctxs[d], node_ctxs[d], nullptr, 0, (size_t)G, (u32*)m->ex[d]->base, m->d_top[d], L->stream));
         }
         if (G > 1 && d == 0) CPB_CUDA(cudaMemcpyAsync(non_leaf_nodes, m->d_top[0], (size_t)(G - 1) * 32, cudaMemcpyDeviceToHost, L->stream));
-        CPB_CUDA(cudaStreamSynchronize(L->stream));
-        return CPB_OK;
+        return S.download();
     };
     std::vector<std::thread> threads;
     for (int d = 0; d < G; d++)

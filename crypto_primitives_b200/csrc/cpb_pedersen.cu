@@ -730,16 +730,50 @@ void cpb_pedersen_ctx_destroy(cpb_pedersen_ctx* c) {
     if (c->stream) { cudaStreamSynchronize(c->stream); cudaStreamDestroy(c->stream); }
     if (c->d_consts) cudaFree(c->d_consts);
     if (c->d_table) cudaFree(c->d_table);
-    c->s_in.release(); c->s_out.release(); c->s_aux.release(); c->s_rand.release();
     delete c;
+}
+
+// ---- the checks each operation's two forms share (the host forms add theirs on host arrays around them)
+static cpb_status check_hash(cpb_pedersen_ctx* c, size_t len, const uint8_t* rnd, size_t n, bool commit) {
+    CPB_TRY(ped_check(c));
+    if (commit) {
+        if (c->n_rand == 0) return fail(CPB_BAD_PARAMS, "context has no randomness generators");
+        if (!rnd && n) return fail(CPB_NULL_POINTER, "null randomness");
+    }
+    return check_len(c, len, commit);
+}
+static cpb_status check_build_ctxs(cpb_pedersen_ctx* leaf, cpb_pedersen_ctx* node, size_t n) {
+    CPB_TRY(ped_check(leaf));
+    CPB_TRY(ped_check(node));
+    if (leaf->device != node->device || leaf->field_id != node->field_id)
+        return fail(CPB_BAD_PARAMS, "leaf and node contexts must share device and curve");
+    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
+    return CPB_OK;
+}
+static cpb_status check_mixed_build(cpb_pedersen_ctx* leaf, cpb_poseidon_ctx* node, size_t n, size_t leaf_len) {
+    CPB_TRY(ped_check(leaf));
+    if (!node) return fail(CPB_NULL_POINTER, "null context");
+    if (cpb_poseidon_ctx_field(node) != leaf->field_id || cpb_poseidon_ctx_device(node) != leaf->device)
+        return fail(CPB_BAD_PARAMS, "the Poseidon field must be the curve's base field, on the same device");
+    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
+    return check_len(leaf, leaf_len, false);
+}
+static cpb_status build_core(cpb_pedersen_ctx* leaf, cpb_pedersen_ctx* node, const uint8_t* leaves, size_t leaf_len, size_t leaf_stride,
+                             size_t n, u32* leaf_nodes, u32* non_leaf_nodes, u32* scratch_64n, cudaStream_t st) {
+    CPB_TRY(launch_hash(leaf, leaves, leaf_len, leaf_stride, nullptr, leaf_nodes, n, 0, st));
+    return pedersen_levels(node, leaf_nodes, n, non_leaf_nodes, scratch_64n, st);
+}
+static cpb_status mixed_build_core(cpb_pedersen_ctx* leaf, cpb_poseidon_ctx* node, const uint8_t* leaves, size_t leaf_len, size_t leaf_stride,
+                                   size_t n, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes, cudaStream_t st) {
+    CPB_TRY(launch_hash(leaf, leaves, leaf_len, leaf_stride, nullptr, (u32*)leaf_nodes, n, 1, st));
+    return cpb_merkle_poseidon_from_digests_dev(node, leaf_nodes, n, non_leaf_nodes, st);
 }
 
 // ---- device-pointer entry points
 cpb_status cpb_pedersen_crh_batch_dev(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, size_t stride, uint64_t* out_xy,
                                       size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(ped_check(c));
-    CPB_TRY(check_len(c, len, false));
+    CPB_TRY(check_hash(c, len, nullptr, n, false));
     DeviceGuard g(c->device);
     return launch_hash(c, in, len, stride, nullptr, (u32*)out_xy, n, 0, (cudaStream_t)stream);
     });
@@ -747,8 +781,7 @@ cpb_status cpb_pedersen_crh_batch_dev(cpb_pedersen_ctx* c, const uint8_t* in, si
 cpb_status cpb_pedersen_crh_x_batch_dev(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, size_t stride, uint64_t* out_x,
                                         size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(ped_check(c));
-    CPB_TRY(check_len(c, len, false));
+    CPB_TRY(check_hash(c, len, nullptr, n, false));
     DeviceGuard g(c->device);
     return launch_hash(c, in, len, stride, nullptr, (u32*)out_x, n, 1, (cudaStream_t)stream);
     });
@@ -756,10 +789,7 @@ cpb_status cpb_pedersen_crh_x_batch_dev(cpb_pedersen_ctx* c, const uint8_t* in, 
 cpb_status cpb_pedersen_commit_batch_dev(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, size_t stride,
                                          const uint8_t* randomness_le32, uint64_t* out_xy, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(ped_check(c));
-    if (c->n_rand == 0) return fail(CPB_BAD_PARAMS, "context has no randomness generators");
-    if (!randomness_le32 && n) return fail(CPB_NULL_POINTER, "null randomness");
-    CPB_TRY(check_len(c, len, true));
+    CPB_TRY(check_hash(c, len, randomness_le32, n, true));
     DeviceGuard g(c->device);
     return launch_hash(c, in, len, stride, randomness_le32, (u32*)out_xy, n, 0, (cudaStream_t)stream);
     });
@@ -777,33 +807,21 @@ cpb_status cpb_merkle_pedersen_build_dev(cpb_pedersen_ctx* leaf, cpb_pedersen_ct
                                          size_t leaf_len, size_t leaf_stride, size_t n, uint64_t* leaf_nodes_xy,
                                          uint64_t* non_leaf_nodes_xy, void* scratch_64n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(ped_check(leaf));
-    CPB_TRY(ped_check(node));
-    if (leaf->device != node->device || leaf->field_id != node->field_id)
-        return fail(CPB_BAD_PARAMS, "leaf and node contexts must share device and curve");
-    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
+    CPB_TRY(check_build_ctxs(leaf, node, n));
     if (!scratch_64n) return fail(CPB_NULL_POINTER, "null scratch");
     CPB_TRY(check_len(leaf, leaf_len, false));
     DeviceGuard g(leaf->device);
-    cudaStream_t st = (cudaStream_t)stream;
-    CPB_TRY(launch_hash(leaf, leaves, leaf_len, leaf_stride, nullptr, (u32*)leaf_nodes_xy, n, 0, st));
-    return pedersen_levels(node, (const u32*)leaf_nodes_xy, n, (u32*)non_leaf_nodes_xy, (u32*)scratch_64n, st);
+    return build_core(leaf, node, leaves, leaf_len, leaf_stride, n, (u32*)leaf_nodes_xy, (u32*)non_leaf_nodes_xy, (u32*)scratch_64n,
+                      (cudaStream_t)stream);
     });
 }
 cpb_status cpb_merkle_mixed_build_dev(cpb_pedersen_ctx* leaf, cpb_poseidon_ctx* node, const uint8_t* leaves, size_t leaf_len,
                                       size_t leaf_stride, size_t n, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes,
                                       void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(ped_check(leaf));
-    if (!node) return fail(CPB_NULL_POINTER, "null context");
-    if (cpb_poseidon_ctx_field(node) != leaf->field_id || cpb_poseidon_ctx_device(node) != leaf->device)
-        return fail(CPB_BAD_PARAMS, "the Poseidon field must be the curve's base field, on the same device");
-    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
-    CPB_TRY(check_len(leaf, leaf_len, false));
+    CPB_TRY(check_mixed_build(leaf, node, n, leaf_len));
     DeviceGuard g(leaf->device);
-    cudaStream_t st = (cudaStream_t)stream;
-    CPB_TRY(launch_hash(leaf, leaves, leaf_len, leaf_stride, nullptr, (u32*)leaf_nodes, n, 1, st));
-    return cpb_merkle_poseidon_from_digests_dev(node, leaf_nodes, n, non_leaf_nodes, stream);
+    return mixed_build_core(leaf, node, leaves, leaf_len, leaf_stride, n, leaf_nodes, non_leaf_nodes, (cudaStream_t)stream);
     });
 }
 
@@ -827,30 +845,20 @@ cpb_status cpb_merkle_mixed_build_sharded_dev(cpb_pedersen_ctx* leaf, cpb_poseid
     });
 }
 
-// ---- host-pointer entry points
+// ---- host-pointer entry points: the _dev form's core on the context arena and stream (HostStage), under the context mutex
 static cpb_status ped_host_hash(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, size_t stride, const uint8_t* rnd,
                                 uint64_t* out, size_t n, int mode, bool commit) {
-    CPB_TRY(ped_check(c));
-    CPB_TRY(check_len(c, len, commit));
+    CPB_TRY(check_hash(c, len, rnd, n, commit));
     if (n == 0) return CPB_OK;
     if ((!in && len) || !out) return fail(CPB_NULL_POINTER, "null buffer");
     if (stride < len) return fail(CPB_BAD_PARAMS, "stride < len");
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    size_t in_b = (n - 1) * stride + len, out_b = n * (mode == 0 ? 64 : 32);
-    CPB_TRY(c->s_in.reserve(in_b ? in_b : 16));
-    CPB_TRY(c->s_out.reserve(out_b));
-    if (in_b) CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, in, in_b, cudaMemcpyHostToDevice, c->stream));
-    const uint8_t* d_rnd = nullptr;
-    if (rnd) {
-        CPB_TRY(c->s_rand.reserve(n * 32));
-        CPB_CUDA(cudaMemcpyAsync(c->s_rand.ptr, rnd, n * 32, cudaMemcpyHostToDevice, c->stream));
-        d_rnd = (const uint8_t*)c->s_rand.ptr;
-    }
-    CPB_TRY(launch_hash(c, (const uint8_t*)c->s_in.ptr, len, stride, d_rnd, (u32*)c->s_out.ptr, n, mode, c->stream));
-    CPB_CUDA(cudaMemcpyAsync(out, c->s_out.ptr, out_b, cudaMemcpyDeviceToHost, c->stream));
-    CPB_CUDA(cudaStreamSynchronize(c->stream));
-    return CPB_OK;
+    HostStage S(c->arena, c->stream);
+    const size_t o_in = S.in(in, (n - 1) * stride + len), o_rnd = S.in(rnd, rnd ? n * 32 : 0), o_out = S.out(out, n * (mode == 0 ? 64 : 32));
+    CPB_TRY(S.upload());
+    CPB_TRY(launch_hash(c, S.at<uint8_t>(o_in), len, stride, rnd ? S.at<uint8_t>(o_rnd) : nullptr, S.at<u32>(o_out), n, mode, c->stream));
+    return S.download();
 }
 cpb_status cpb_pedersen_crh_batch(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, size_t stride, uint64_t* out_xy, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
@@ -865,9 +873,6 @@ cpb_status cpb_pedersen_crh_x_batch(cpb_pedersen_ctx* c, const uint8_t* in, size
 cpb_status cpb_pedersen_commit_batch(cpb_pedersen_ctx* c, const uint8_t* in, size_t len, size_t stride,
                                      const uint8_t* randomness_le32, uint64_t* out_xy, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(ped_check(c));
-    if (c->n_rand == 0) return fail(CPB_BAD_PARAMS, "context has no randomness generators");
-    if (!randomness_le32 && n) return fail(CPB_NULL_POINTER, "null randomness");
     return ped_host_hash(c, in, len, stride, randomness_le32, out_xy, n, 0, true);
     });
 }
@@ -878,14 +883,11 @@ cpb_status cpb_pedersen_two_to_one_batch(cpb_pedersen_ctx* c, const uint64_t* ch
     if (!children_xy || !out_xy) return fail(CPB_NULL_POINTER, "null buffer");
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    CPB_TRY(c->s_in.reserve(n * 128));
-    CPB_TRY(c->s_aux.reserve(n * 128));
-    CPB_TRY(c->s_out.reserve(n * 64));
-    CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, children_xy, n * 128, cudaMemcpyHostToDevice, c->stream));
-    CPB_TRY(two_to_one_dev(c, (const u32*)c->s_in.ptr, (u32*)c->s_out.ptr, n, (u32*)c->s_aux.ptr, c->stream));
-    CPB_CUDA(cudaMemcpyAsync(out_xy, c->s_out.ptr, n * 64, cudaMemcpyDeviceToHost, c->stream));
-    CPB_CUDA(cudaStreamSynchronize(c->stream));
-    return CPB_OK;
+    HostStage S(c->arena, c->stream);
+    const size_t o_in = S.in(children_xy, n * 128), o_tmp = S.dev(n * 128), o_out = S.out(out_xy, n * 64);
+    CPB_TRY(S.upload());
+    CPB_TRY(two_to_one_dev(c, S.at<u32>(o_in), S.at<u32>(o_out), n, S.at<u32>(o_tmp), c->stream));
+    return S.download();
     });
 }
 cpb_status cpb_merkle_pedersen_build(cpb_pedersen_ctx* leaf, cpb_pedersen_ctx* node, const uint8_t* leaves, size_t leaf_len,
@@ -895,21 +897,17 @@ cpb_status cpb_merkle_pedersen_build(cpb_pedersen_ctx* leaf, cpb_pedersen_ctx* n
     CPB_TRY(ped_check(node));
     if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
     if ((!leaves && leaf_len) || !leaf_nodes_xy || !non_leaf_nodes_xy) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(check_build_ctxs(leaf, node, n));
+    CPB_TRY(check_len(leaf, leaf_len, false));
     std::lock_guard<std::mutex> lk(leaf->mu);
     DeviceGuard g(leaf->device);
-    CPB_TRY(leaf->s_in.reserve(n * leaf_len ? n * leaf_len : 16));
-    CPB_TRY(leaf->s_out.reserve(n * 64 + (n - 1) * 64));
-    CPB_TRY(leaf->s_aux.reserve(n * 64));
-    cudaStream_t st = leaf->stream;
-    u32* d_leaf = (u32*)leaf->s_out.ptr;
-    u32* d_nodes = d_leaf + 16 * n;
-    if (n * leaf_len) CPB_CUDA(cudaMemcpyAsync(leaf->s_in.ptr, leaves, n * leaf_len, cudaMemcpyHostToDevice, st));
-    CPB_TRY(cpb_merkle_pedersen_build_dev(leaf, node, (const uint8_t*)leaf->s_in.ptr, leaf_len, leaf_len, n, (uint64_t*)d_leaf,
-                                          (uint64_t*)d_nodes, leaf->s_aux.ptr, st));
-    CPB_CUDA(cudaMemcpyAsync(leaf_nodes_xy, d_leaf, n * 64, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaMemcpyAsync(non_leaf_nodes_xy, d_nodes, (n - 1) * 64, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    HostStage S(leaf->arena, leaf->stream);
+    const size_t o_in = S.in(leaves, n * leaf_len), o_leaf = S.out(leaf_nodes_xy, n * 64), o_nodes = S.out(non_leaf_nodes_xy, (n - 1) * 64),
+                 o_tmp = S.dev(n * 64);
+    CPB_TRY(S.upload());
+    CPB_TRY(build_core(leaf, node, S.at<uint8_t>(o_in), leaf_len, leaf_len, n, S.at<u32>(o_leaf), S.at<u32>(o_nodes), S.at<u32>(o_tmp),
+                       leaf->stream));
+    return S.download();
     });
 }
 cpb_status cpb_merkle_mixed_build(cpb_pedersen_ctx* leaf, cpb_poseidon_ctx* node, const uint8_t* leaves, size_t leaf_len,
@@ -919,20 +917,15 @@ cpb_status cpb_merkle_mixed_build(cpb_pedersen_ctx* leaf, cpb_poseidon_ctx* node
     if (!node) return fail(CPB_NULL_POINTER, "null context");
     if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
     if ((!leaves && leaf_len) || !leaf_nodes || !non_leaf_nodes) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(check_mixed_build(leaf, node, n, leaf_len));
     std::lock_guard<std::mutex> lk(leaf->mu);
     DeviceGuard g(leaf->device);
-    CPB_TRY(leaf->s_in.reserve(n * leaf_len ? n * leaf_len : 16));
-    CPB_TRY(leaf->s_out.reserve(n * 32 + (n - 1) * 32));
-    cudaStream_t st = leaf->stream;
-    u32* d_leaf = (u32*)leaf->s_out.ptr;
-    u32* d_nodes = d_leaf + 8 * n;
-    if (n * leaf_len) CPB_CUDA(cudaMemcpyAsync(leaf->s_in.ptr, leaves, n * leaf_len, cudaMemcpyHostToDevice, st));
-    CPB_TRY(cpb_merkle_mixed_build_dev(leaf, node, (const uint8_t*)leaf->s_in.ptr, leaf_len, leaf_len, n, (uint64_t*)d_leaf,
-                                       (uint64_t*)d_nodes, st));
-    CPB_CUDA(cudaMemcpyAsync(leaf_nodes, d_leaf, n * 32, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaMemcpyAsync(non_leaf_nodes, d_nodes, (n - 1) * 32, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    HostStage S(leaf->arena, leaf->stream);
+    const size_t o_in = S.in(leaves, n * leaf_len), o_leaf = S.out(leaf_nodes, n * 32), o_nodes = S.out(non_leaf_nodes, (n - 1) * 32);
+    CPB_TRY(S.upload());
+    CPB_TRY(mixed_build_core(leaf, node, S.at<uint8_t>(o_in), leaf_len, leaf_len, n, S.at<uint64_t>(o_leaf), S.at<uint64_t>(o_nodes),
+                             leaf->stream));
+    return S.download();
     });
 }
 
@@ -948,7 +941,7 @@ struct cpb_bowe_hopwood_ctx {
     u32* d_table = nullptr;
     cudaStream_t stream = nullptr;
     std::mutex mu;
-    Scratch s_in, s_out, s_aux;
+    Scratch arena;      // the host-pointer entry points' device copies (HostStage), under mu
 };
 
 namespace {
@@ -1081,7 +1074,6 @@ void cpb_bowe_hopwood_ctx_destroy(cpb_bowe_hopwood_ctx* c) {
     if (c->d_consts) cudaFree(c->d_consts);
     if (c->d_table3) cudaFree(c->d_table3);
     if (c->d_table) cudaFree(c->d_table);
-    c->s_in.release(); c->s_out.release(); c->s_aux.release();
     delete c;
 }
 
@@ -1114,14 +1106,11 @@ cpb_status cpb_bowe_hopwood_crh_batch(cpb_bowe_hopwood_ctx* c, const uint8_t* in
     if (stride < len) return fail(CPB_BAD_PARAMS, "stride < len");
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    size_t in_b = (n - 1) * stride + len;
-    CPB_TRY(c->s_in.reserve(in_b ? in_b : 16));
-    CPB_TRY(c->s_out.reserve(n * 32));
-    if (in_b) CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, in, in_b, cudaMemcpyHostToDevice, c->stream));
-    CPB_TRY(bh_launch(c, (const uint8_t*)c->s_in.ptr, len, stride, (u32*)c->s_out.ptr, n, c->stream));
-    CPB_CUDA(cudaMemcpyAsync(out_x, c->s_out.ptr, n * 32, cudaMemcpyDeviceToHost, c->stream));
-    CPB_CUDA(cudaStreamSynchronize(c->stream));
-    return CPB_OK;
+    HostStage S(c->arena, c->stream);
+    const size_t o_in = S.in(in, (n - 1) * stride + len), o_out = S.out(out_x, n * 32);
+    CPB_TRY(S.upload());
+    CPB_TRY(bh_launch(c, S.at<uint8_t>(o_in), len, stride, S.at<u32>(o_out), n, c->stream));
+    return S.download();
     });
 }
 cpb_status cpb_bowe_hopwood_two_to_one_batch(cpb_bowe_hopwood_ctx* c, const uint64_t* children_x, uint64_t* out_x, size_t n) {
@@ -1131,14 +1120,11 @@ cpb_status cpb_bowe_hopwood_two_to_one_batch(cpb_bowe_hopwood_ctx* c, const uint
     if (!children_x || !out_x) return fail(CPB_NULL_POINTER, "null buffer");
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    CPB_TRY(c->s_in.reserve(n * 64));
-    CPB_TRY(c->s_aux.reserve(n * bh_two_to_one_stride(c)));
-    CPB_TRY(c->s_out.reserve(n * 32));
-    CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, children_x, n * 64, cudaMemcpyHostToDevice, c->stream));
-    CPB_TRY(bh_two_to_one_dev(c, (const u32*)c->s_in.ptr, (u32*)c->s_out.ptr, n, (uint8_t*)c->s_aux.ptr, c->stream));
-    CPB_CUDA(cudaMemcpyAsync(out_x, c->s_out.ptr, n * 32, cudaMemcpyDeviceToHost, c->stream));
-    CPB_CUDA(cudaStreamSynchronize(c->stream));
-    return CPB_OK;
+    HostStage S(c->arena, c->stream);
+    const size_t o_in = S.in(children_x, n * 64), o_tmp = S.dev(n * bh_two_to_one_stride(c)), o_out = S.out(out_x, n * 32);
+    CPB_TRY(S.upload());
+    CPB_TRY(bh_two_to_one_dev(c, S.at<u32>(o_in), S.at<u32>(o_out), n, S.at<uint8_t>(o_tmp), c->stream));
+    return S.download();
     });
 }
 

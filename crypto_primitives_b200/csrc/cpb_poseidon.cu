@@ -552,23 +552,6 @@ cpb_status check_offsets(const uint64_t* offsets, size_t n) {
     return CPB_OK;
 }
 
-// Copies a ragged host batch into `buf`: the n + 1 offsets at d_off, then values[offsets[0] .. offsets[n]) at d_val (so the
-// device values start at index vbase = offsets[0]).  `front` bytes at the start of buf are left to the caller.  `unit`: bytes per
-// offset step (32 for field elements, 1 for byte strings, 0 to copy offsets only).
-cpb_status stage_ragged(Scratch& buf, size_t front, const void* values, const uint64_t* offsets, size_t n, cudaStream_t st,
-                        u64*& d_off, u32*& d_val, size_t unit = 32) {
-    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t b_off = (n + 1) * 8, b_val = (size_t)(offsets[n] - offsets[0]) * unit;
-    const size_t o_off = up(front), o_val = o_off + up(b_off);
-    CPB_TRY(buf.reserve(o_val + (b_val ? b_val : 32)));
-    char* d = (char*)buf.ptr;
-    d_off = (u64*)(d + o_off);
-    d_val = (u32*)(d + o_val);
-    CPB_CUDA(cudaMemcpyAsync(d_off, offsets, b_off, cudaMemcpyHostToDevice, st));
-    if (b_val) CPB_CUDA(cudaMemcpyAsync(d_val, (const char*)values + unit * offsets[0], b_val, cudaMemcpyHostToDevice, st));
-    return CPB_OK;
-}
-
 }  // namespace cpb
 
 // ------------------------------------------------------------------------------ C ABI
@@ -621,31 +604,6 @@ cpb_status cpb_field_modulus(int field_id, uint64_t out[4]) {
     });
 }
 
-static cpb_status field_convert(int field_id, int device, const uint64_t* in, uint64_t* out, size_t n, int to_mont) {
-    if (!host::element_field_modulus(field_id)) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
-    if (n == 0) return CPB_OK;
-    if (!in || !out) return fail(CPB_NULL_POINTER, "null buffer");
-    DeviceGuard g(device);
-    if (!g.ok) return fail(CPB_NO_DEVICE, "cudaSetDevice(%d) failed", device);
-    u32* d = nullptr;
-    CPB_CUDA(cudaMalloc(&d, n * 32));
-    cudaError_t e = cudaMemcpy(d, in, n * 32, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        int grid = (int)((n + 127) / 128);
-        switch (field_id) {
-            case 0: k_field_convert<Bls12_381_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
-            case 1: k_field_convert<Bn254_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
-            case 2: k_field_convert<Jubjub_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
-            case 3: k_field_convert<Bls12_377_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
-            case 4: k_field_convert<Ed_On_Bls12_377_Fr><<<grid, 128>>>(d, d, (long)n, to_mont); break;
-        }
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpy(out, d, n * 32, cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    if (e != cudaSuccess) return fail(CPB_CUDA_ERROR, "field conversion failed: %s", cudaGetErrorString(e));
-    return CPB_OK;
-}
 static cpb_status field_convert_dev(int field_id, int device, const uint64_t* in, uint64_t* out, size_t n, int to_mont, void* stream) {
     if (!host::element_field_modulus(field_id)) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
     if (n == 0) return CPB_OK;
@@ -670,6 +628,20 @@ static cpb_status field_convert_dev(int field_id, int device, const uint64_t* in
         left -= m; off += m;
     }
     return CPB_OK;
+}
+// The host form: the device form on a local arena, on the legacy stream.
+static cpb_status field_convert(int field_id, int device, const uint64_t* in, uint64_t* out, size_t n, int to_mont) {
+    if (!host::element_field_modulus(field_id)) return fail(CPB_BAD_PARAMS, "unknown field id %d", field_id);
+    if (n == 0) return CPB_OK;
+    if (!in || !out) return fail(CPB_NULL_POINTER, "null buffer");
+    DeviceGuard g(device);
+    if (!g.ok) return fail(CPB_NO_DEVICE, "cudaSetDevice(%d) failed", device);
+    Scratch arena;
+    HostStage S(arena, nullptr);
+    const size_t o_in = S.in(in, n * 32), o_out = S.out(out, n * 32);
+    CPB_TRY(S.upload());
+    CPB_TRY(field_convert_dev(field_id, device, S.at<uint64_t>(o_in), S.at<uint64_t>(o_out), n, to_mont, nullptr));
+    return S.download();
 }
 cpb_status cpb_field_to_montgomery_dev(int field_id, int device, const uint64_t* in, uint64_t* out, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status { return field_convert_dev(field_id, device, in, out, n, 1, stream); });
@@ -814,13 +786,45 @@ void cpb_poseidon_ctx_destroy(cpb_poseidon_ctx* c) {
     if (c->d_consts) cudaFree(c->d_consts);
     for (auto& s : c->side)
         if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-    c->s_in.release(); c->s_out.release(); c->s_aux.release();
     delete c;
 }
 
 int cpb_poseidon_ctx_is_sparse(const cpb_poseidon_ctx* c) { return c ? c->sched.sparse : 0; }
 int cpb_poseidon_ctx_field(const cpb_poseidon_ctx* c) { return c ? c->field_id : -1; }
 int cpb_poseidon_ctx_device(const cpb_poseidon_ctx* c) { return c ? c->device : -1; }
+
+// ---- the checks each operation's two forms share (the host forms add theirs on host arrays around them)
+static cpb_status check_compress(cpb_poseidon_ctx* c) {
+    CPB_TRY(check_ctx(c));
+    if (c->dev.rate < 2)   // two absorbs then one squeeze = one permutation only when rate >= 2
+        return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    return CPB_OK;
+}
+static cpb_status check_from_digests(cpb_poseidon_ctx* node, size_t n) {
+    CPB_TRY(check_ctx(node));
+    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
+    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    return CPB_OK;
+}
+static cpb_status check_tree_ctxs(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, size_t n) {
+    CPB_TRY(check_ctx(leaf));
+    CPB_TRY(check_ctx(node));
+    if (leaf->device != node->device || leaf->field_id != node->field_id)
+        return fail(CPB_BAD_PARAMS, "leaf and node contexts must share device and field");
+    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
+    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    return CPB_OK;
+}
+
+static cpb_status check_verify_ctxs(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, size_t path_len) {
+    CPB_TRY(check_ctx(leaf));
+    CPB_TRY(check_ctx(node));
+    if (leaf->device != node->device || leaf->field_id != node->field_id || leaf->dev.t != node->dev.t)
+        return fail(CPB_UNSUPPORTED, "leaf and node contexts must share device, field and state width");
+    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    if (path_len > 62) return fail(CPB_BAD_PARAMS, "path too long");
+    return CPB_OK;
+}
 
 // ---- device-pointer entry points
 cpb_status cpb_poseidon_permute_batch_dev(cpb_poseidon_ctx* c, const uint64_t* in, uint64_t* out, size_t n, void* stream) {
@@ -850,12 +854,7 @@ cpb_status cpb_merkle_poseidon_verify_batch_dev(cpb_poseidon_ctx* leaf, cpb_pose
                                                 const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes,
                                                 uint8_t* ok, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_ctx(leaf));
-    CPB_TRY(check_ctx(node));
-    if (leaf->device != node->device || leaf->field_id != node->field_id || leaf->dev.t != node->dev.t)
-        return fail(CPB_UNSUPPORTED, "leaf and node contexts must share device, field and state width");
-    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
-    if (path_len > 62) return fail(CPB_BAD_PARAMS, "path too long");
+    CPB_TRY(check_verify_ctxs(leaf, node, path_len));
     DeviceGuard g(leaf->device);
     return launch_verify(leaf, node, (const u32*)root, (const u32*)leaves, leaf_len, (const u32*)leaf_sibling_hashes,
                          (const u32*)auth_paths, (int)path_len, (const unsigned long long*)leaf_indexes, ok, n, (cudaStream_t)stream);
@@ -863,9 +862,7 @@ cpb_status cpb_merkle_poseidon_verify_batch_dev(cpb_poseidon_ctx* leaf, cpb_pose
 }
 cpb_status cpb_poseidon_compress_batch_dev(cpb_poseidon_ctx* c, const uint64_t* pairs, uint64_t* out, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_ctx(c));
-    if (c->dev.rate < 2)   // two absorbs then one squeeze = one permutation only when rate >= 2
-        return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    CPB_TRY(check_compress(c));
     DeviceGuard g(c->device);
     return launch_crh(c, (const u32*)pairs, 2, (u32*)out, n, (cudaStream_t)stream);
     });
@@ -873,9 +870,7 @@ cpb_status cpb_poseidon_compress_batch_dev(cpb_poseidon_ctx* c, const uint64_t* 
 cpb_status cpb_merkle_poseidon_from_digests_dev(cpb_poseidon_ctx* node, const uint64_t* leaf_digests, size_t n,
                                                 uint64_t* non_leaf_nodes, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_ctx(node));
-    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
-    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    CPB_TRY(check_from_digests(node, n));
     DeviceGuard g(node->device);
     return merkle_build_streams(node, node, nullptr, 0, n, (u32*)leaf_digests, (u32*)non_leaf_nodes, (cudaStream_t)stream);
     });
@@ -884,45 +879,44 @@ cpb_status cpb_merkle_poseidon_build_dev(cpb_poseidon_ctx* leaf, cpb_poseidon_ct
                                          size_t leaf_len, size_t n, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes,
                                          void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_ctx(leaf));
-    CPB_TRY(check_ctx(node));
-    if (leaf->device != node->device || leaf->field_id != node->field_id)
-        return fail(CPB_BAD_PARAMS, "leaf and node contexts must share device and field");
-    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
-    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    CPB_TRY(check_tree_ctxs(leaf, node, n));
     DeviceGuard g(leaf->device);
     return merkle_build_streams(leaf, node, (const u32*)leaves, leaf_len, n, (u32*)leaf_nodes, (u32*)non_leaf_nodes,
                                 (cudaStream_t)stream);
     });
 }
 
-// ---- host-pointer entry points: H2D, launch, D2H on the context stream
-static cpb_status host_roundtrip_crh(cpb_poseidon_ctx* c, const uint64_t* in, size_t in_elems_per, size_t len,
-                                     uint64_t* out, size_t out_elems_per, size_t n, int mode) {
-    CPB_TRY(check_ctx(c));
-    if (n == 0) return CPB_OK;
-    if ((!in && in_elems_per) || !out) return fail(CPB_NULL_POINTER, "null buffer");
-    std::lock_guard<std::mutex> lk(c->mu);
-    DeviceGuard g(c->device);
-    size_t in_b = n * in_elems_per * 32, out_b = n * out_elems_per * 32;
-    CPB_TRY(c->s_in.reserve(in_b ? in_b : 32));
-    CPB_TRY(c->s_out.reserve(out_b));
-    if (in_b) CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, in, in_b, cudaMemcpyHostToDevice, c->stream));
-    if (mode == 0) CPB_TRY(launch_crh(c, (const u32*)c->s_in.ptr, len, (u32*)c->s_out.ptr, n, c->stream));
-    else CPB_TRY(launch_permute(c, (const u32*)c->s_in.ptr, (u32*)c->s_out.ptr, n, c->stream));
-    CPB_CUDA(cudaMemcpyAsync(out, c->s_out.ptr, out_b, cudaMemcpyDeviceToHost, c->stream));
-    CPB_CUDA(cudaStreamSynchronize(c->stream));
-    return CPB_OK;
-}
+// ---- host-pointer entry points: the _dev form's core on the context arena and stream (HostStage), under the context mutex
 cpb_status cpb_poseidon_permute_batch(cpb_poseidon_ctx* c, const uint64_t* in, uint64_t* out, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
     CPB_TRY(check_ctx(c));
-    return host_roundtrip_crh(c, in, (size_t)c->dev.t, 0, out, (size_t)c->dev.t, n, 1);
+    if (n == 0) return CPB_OK;
+    if (!in || !out) return fail(CPB_NULL_POINTER, "null buffer");
+    std::lock_guard<std::mutex> lk(c->mu);
+    DeviceGuard g(c->device);
+    HostStage S(c->arena, c->stream);
+    const size_t b = n * (size_t)c->dev.t * 32, o_in = S.in(in, b), o_out = S.out(out, b);
+    CPB_TRY(S.upload());
+    CPB_TRY(launch_permute(c, S.at<u32>(o_in), S.at<u32>(o_out), n, c->stream));
+    return S.download();
     });
+}
+// CRH, sponge and two-to-one: n inputs of len elements in, n_squeeze elements out each (checked by the caller).
+static cpb_status sponge_host(cpb_poseidon_ctx* c, const uint64_t* in, size_t len, uint64_t* out, size_t n_squeeze, size_t n) {
+    std::lock_guard<std::mutex> lk(c->mu);
+    DeviceGuard g(c->device);
+    HostStage S(c->arena, c->stream);
+    const size_t o_in = S.in(in, n * len * 32), o_out = S.out(out, n * n_squeeze * 32);
+    CPB_TRY(S.upload());
+    CPB_TRY(launch_crh(c, S.at<u32>(o_in), len, S.at<u32>(o_out), n, c->stream, n_squeeze));
+    return S.download();
 }
 cpb_status cpb_poseidon_crh_batch(cpb_poseidon_ctx* c, const uint64_t* in, size_t len, uint64_t* out, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    return host_roundtrip_crh(c, in, len, len, out, 1, n, 0);
+    CPB_TRY(check_ctx(c));
+    if (n == 0) return CPB_OK;
+    if ((!in && len) || !out) return fail(CPB_NULL_POINTER, "null buffer");
+    return sponge_host(c, in, len, out, 1, n);
     });
 }
 cpb_status cpb_poseidon_sponge_batch(cpb_poseidon_ctx* c, const uint64_t* in, size_t len, uint64_t* out, size_t n_squeeze, size_t n) {
@@ -930,16 +924,7 @@ cpb_status cpb_poseidon_sponge_batch(cpb_poseidon_ctx* c, const uint64_t* in, si
     CPB_TRY(check_ctx(c));
     if (n == 0 || n_squeeze == 0) return CPB_OK;
     if ((!in && len) || !out) return fail(CPB_NULL_POINTER, "null buffer");
-    std::lock_guard<std::mutex> lk(c->mu);
-    DeviceGuard g(c->device);
-    size_t in_b = n * len * 32, out_b = n * n_squeeze * 32;
-    CPB_TRY(c->s_in.reserve(in_b ? in_b : 32));
-    CPB_TRY(c->s_out.reserve(out_b));
-    if (in_b) CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, in, in_b, cudaMemcpyHostToDevice, c->stream));
-    CPB_TRY(launch_crh(c, (const u32*)c->s_in.ptr, len, (u32*)c->s_out.ptr, n, c->stream, n_squeeze));
-    CPB_CUDA(cudaMemcpyAsync(out, c->s_out.ptr, out_b, cudaMemcpyDeviceToHost, c->stream));
-    CPB_CUDA(cudaStreamSynchronize(c->stream));
-    return CPB_OK;
+    return sponge_host(c, in, len, out, n_squeeze, n);
     });
 }
 cpb_status cpb_merkle_poseidon_verify_batch(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, const uint64_t* root,
@@ -952,34 +937,24 @@ cpb_status cpb_merkle_poseidon_verify_batch(cpb_poseidon_ctx* leaf, cpb_poseidon
     if (n == 0) return CPB_OK;
     if (!root || (!leaves && leaf_len) || !leaf_sibling_hashes || (!auth_paths && path_len) || !leaf_indexes || !ok)
         return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(check_verify_ctxs(leaf, node, path_len));
     std::lock_guard<std::mutex> lk(leaf->mu);
     DeviceGuard g(leaf->device);
-    size_t b_root = 32, b_leaves = n * leaf_len * 32, b_sib = n * 32, b_path = n * path_len * 32, b_idx = n * 8;
-    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    size_t o_leaves = up(b_root), o_sib = o_leaves + up(b_leaves), o_path = o_sib + up(b_sib), o_idx = o_path + up(b_path),
-           total = o_idx + up(b_idx);
-    CPB_TRY(leaf->s_in.reserve(total));
-    CPB_TRY(leaf->s_out.reserve(n));
-    char* d = (char*)leaf->s_in.ptr;
-    cudaStream_t st = leaf->stream;
-    CPB_CUDA(cudaMemcpyAsync(d, root, b_root, cudaMemcpyHostToDevice, st));
-    if (b_leaves) CPB_CUDA(cudaMemcpyAsync(d + o_leaves, leaves, b_leaves, cudaMemcpyHostToDevice, st));
-    CPB_CUDA(cudaMemcpyAsync(d + o_sib, leaf_sibling_hashes, b_sib, cudaMemcpyHostToDevice, st));
-    if (b_path) CPB_CUDA(cudaMemcpyAsync(d + o_path, auth_paths, b_path, cudaMemcpyHostToDevice, st));
-    CPB_CUDA(cudaMemcpyAsync(d + o_idx, leaf_indexes, b_idx, cudaMemcpyHostToDevice, st));
-    CPB_TRY(cpb_merkle_poseidon_verify_batch_dev(leaf, node, (const uint64_t*)d, (const uint64_t*)(d + o_leaves), leaf_len,
-                                                 (const uint64_t*)(d + o_sib), (const uint64_t*)(d + o_path), path_len,
-                                                 (const uint64_t*)(d + o_idx), (uint8_t*)leaf->s_out.ptr, n, st));
-    CPB_CUDA(cudaMemcpyAsync(ok, leaf->s_out.ptr, n, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    HostStage S(leaf->arena, leaf->stream);
+    const size_t o_root = S.in(root, 32), o_leaves = S.in(leaves, n * leaf_len * 32), o_sib = S.in(leaf_sibling_hashes, n * 32),
+                 o_path = S.in(auth_paths, n * path_len * 32), o_idx = S.in(leaf_indexes, n * 8), o_ok = S.out(ok, n);
+    CPB_TRY(S.upload());
+    CPB_TRY(launch_verify(leaf, node, S.at<u32>(o_root), S.at<u32>(o_leaves), leaf_len, S.at<u32>(o_sib), S.at<u32>(o_path), (int)path_len,
+                          S.at<unsigned long long>(o_idx), S.at<uint8_t>(o_ok), n, leaf->stream));
+    return S.download();
     });
 }
 cpb_status cpb_poseidon_compress_batch(cpb_poseidon_ctx* c, const uint64_t* pairs, uint64_t* out, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_ctx(c));
-    if (c->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
-    return host_roundtrip_crh(c, pairs, 2, 2, out, 1, n, 0);
+    CPB_TRY(check_compress(c));
+    if (n == 0) return CPB_OK;
+    if (!pairs || !out) return fail(CPB_NULL_POINTER, "null buffer");
+    return sponge_host(c, pairs, 2, out, 1, n);
     });
 }
 
@@ -989,18 +964,19 @@ cpb_status cpb_merkle_poseidon_from_digests(cpb_poseidon_ctx* node, const uint64
     CPB_TRY(check_ctx(node));
     if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
     if (!leaf_digests || !non_leaf_nodes) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(check_from_digests(node, n));
     std::lock_guard<std::mutex> lk(node->mu);
     DeviceGuard g(node->device);
-    CPB_TRY(node->s_in.reserve(n * 32));
-    CPB_TRY(node->s_out.reserve((n - 1) * 32));
-    CPB_CUDA(cudaMemcpyAsync(node->s_in.ptr, leaf_digests, n * 32, cudaMemcpyHostToDevice, node->stream));
-    CPB_TRY(cpb_merkle_poseidon_from_digests_dev(node, (const uint64_t*)node->s_in.ptr, n, (uint64_t*)node->s_out.ptr, node->stream));
-    CPB_CUDA(cudaMemcpyAsync(non_leaf_nodes, node->s_out.ptr, (n - 1) * 32, cudaMemcpyDeviceToHost, node->stream));
-    CPB_CUDA(cudaStreamSynchronize(node->stream));
-    return CPB_OK;
+    HostStage S(node->arena, node->stream);
+    const size_t o_in = S.in(leaf_digests, n * 32), o_out = S.out(non_leaf_nodes, (n - 1) * 32);
+    CPB_TRY(S.upload());
+    CPB_TRY(merkle_build_streams(node, node, nullptr, 0, n, S.at<u32>(o_in), S.at<u32>(o_out), node->stream));
+    return S.download();
     });
 }
 
+// The leaves go in and the levels come out through MerkleHost (subtree streams, overlapped with hashing): the stage only lays out the
+// three device buffers and synchronises.
 cpb_status cpb_merkle_poseidon_build(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, const uint64_t* leaves,
                                      size_t leaf_len, size_t n, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes) {
     return cpb::guarded([&]() -> cpb_status {
@@ -1008,21 +984,16 @@ cpb_status cpb_merkle_poseidon_build(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* n
     CPB_TRY(check_ctx(node));
     if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
     if ((!leaves && leaf_len) || !leaf_nodes || !non_leaf_nodes) return fail(CPB_NULL_POINTER, "null buffer");
+    CPB_TRY(check_tree_ctxs(leaf, node, n));
     std::lock_guard<std::mutex> lk(leaf->mu);
     DeviceGuard g(leaf->device);
-    size_t in_b = n * leaf_len * 32;
-    CPB_TRY(leaf->s_in.reserve(in_b ? in_b : 32));
-    CPB_TRY(leaf->s_out.reserve(n * 32));
-    CPB_TRY(leaf->s_aux.reserve((n - 1) * 32));
-    cudaStream_t st = leaf->stream;
-    if (leaf->device != node->device || leaf->field_id != node->field_id)
-        return fail(CPB_BAD_PARAMS, "leaf and node contexts must share device and field");
-    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
+    HostStage S(leaf->arena, leaf->stream);
+    const size_t o_in = S.dev(n * leaf_len * 32), o_leaf = S.dev(n * 32), o_nodes = S.dev((n - 1) * 32);
+    CPB_TRY(S.upload());
     MerkleHost H;
     H.leaves = (const u32*)leaves; H.leaf_nodes = (u32*)leaf_nodes; H.nodes = (u32*)non_leaf_nodes;
-    CPB_TRY(merkle_build_streams(leaf, node, (const u32*)leaf->s_in.ptr, leaf_len, n, (u32*)leaf->s_out.ptr, (u32*)leaf->s_aux.ptr, st, &H));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    CPB_TRY(merkle_build_streams(leaf, node, S.at<u32>(o_in), leaf_len, n, S.at<u32>(o_leaf), S.at<u32>(o_nodes), leaf->stream, &H));
+    return S.download();
     });
 }
 
@@ -1049,28 +1020,16 @@ cpb_status cpb_poseidon_sponge_ragged_batch(cpb_poseidon_ctx* c, const uint64_t*
     if (!values && offsets[n] != offsets[0]) return fail(CPB_NULL_POINTER, "null values");
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    u64* d_off = nullptr;
-    u32* d_val = nullptr;
-    CPB_TRY(stage_ragged(c->s_in, 0, values, offsets, n, c->stream, d_off, d_val));
-    CPB_TRY(c->s_out.reserve(n * n_squeeze * 32));
-    CPB_TRY(launch_crh_ragged(c, d_val, offsets[0], d_off, (u32*)c->s_out.ptr, n, n_squeeze, c->stream));
-    CPB_CUDA(cudaMemcpyAsync(out, c->s_out.ptr, n * n_squeeze * 32, cudaMemcpyDeviceToHost, c->stream));
-    CPB_CUDA(cudaStreamSynchronize(c->stream));
-    return CPB_OK;
+    HostStage S(c->arena, c->stream);
+    const size_t o_off = S.in(offsets, (n + 1) * 8), o_val = S.in(values + 4 * offsets[0], (offsets[n] - offsets[0]) * 32),
+                 o_out = S.out(out, n * n_squeeze * 32);
+    CPB_TRY(S.upload());
+    CPB_TRY(launch_crh_ragged(c, S.at<u32>(o_val), offsets[0], S.at<u64>(o_off), S.at<u32>(o_out), n, n_squeeze, c->stream));
+    return S.download();
     });
 }
 cpb_status cpb_poseidon_crh_ragged_batch(cpb_poseidon_ctx* c, const uint64_t* values, const uint64_t* offsets, uint64_t* out, size_t n) {
     return cpb_poseidon_sponge_ragged_batch(c, values, offsets, out, 1, n);
-}
-
-static cpb_status check_tree_ctxs(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, size_t n) {
-    CPB_TRY(check_ctx(leaf));
-    CPB_TRY(check_ctx(node));
-    if (leaf->device != node->device || leaf->field_id != node->field_id)
-        return fail(CPB_BAD_PARAMS, "leaf and node contexts must share device and field");
-    if (!pow2_gt1(n)) return fail(CPB_NOT_POW2, "leaves.len() should be power of two and greater than one (got %zu)", n);
-    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
-    return CPB_OK;
 }
 
 // The ragged leaf hash, then the from-digests build (subtree streams and tree-top kernel included).
@@ -1095,29 +1054,18 @@ cpb_status cpb_merkle_poseidon_build_ragged(cpb_poseidon_ctx* leaf, cpb_poseidon
     std::lock_guard<std::mutex> lk(leaf->mu);
     DeviceGuard g(leaf->device);
     cudaStream_t st = leaf->stream;
-    u64* d_off = nullptr;
-    u32* d_val = nullptr;
-    CPB_TRY(stage_ragged(leaf->s_in, 0, values, offsets, n, st, d_off, d_val));
-    CPB_TRY(leaf->s_out.reserve(n * 32));
-    CPB_TRY(leaf->s_aux.reserve((n - 1) * 32));
-    CPB_TRY(launch_crh_ragged(leaf, d_val, offsets[0], d_off, (u32*)leaf->s_out.ptr, n, 1, st));
+    HostStage S(leaf->arena, st);
+    const size_t o_off = S.in(offsets, (n + 1) * 8), o_val = S.in(values + 4 * offsets[0], (offsets[n] - offsets[0]) * 32),
+                 o_leaf = S.dev(n * 32), o_nodes = S.dev((n - 1) * 32);
+    CPB_TRY(S.upload());
+    CPB_TRY(launch_crh_ragged(leaf, S.at<u32>(o_val), offsets[0], S.at<u64>(o_off), S.at<u32>(o_leaf), n, 1, st));
     MerkleHost H;                        // no leaves to copy in: the subtree streams copy the digests and levels out
     H.leaf_nodes = (u32*)leaf_nodes; H.nodes = (u32*)non_leaf_nodes;
-    CPB_TRY(merkle_build_streams(node, node, nullptr, 0, n, (u32*)leaf->s_out.ptr, (u32*)leaf->s_aux.ptr, st, &H));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    CPB_TRY(merkle_build_streams(node, node, nullptr, 0, n, S.at<u32>(o_leaf), S.at<u32>(o_nodes), st, &H));
+    return S.download();
     });
 }
 
-static cpb_status check_verify_ctxs(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, size_t path_len) {
-    CPB_TRY(check_ctx(leaf));
-    CPB_TRY(check_ctx(node));
-    if (leaf->device != node->device || leaf->field_id != node->field_id || leaf->dev.t != node->dev.t)
-        return fail(CPB_UNSUPPORTED, "leaf and node contexts must share device, field and state width");
-    if (node->dev.rate < 2) return fail(CPB_UNSUPPORTED, "two-to-one with rate < 2 not supported");
-    if (path_len > 62) return fail(CPB_BAD_PARAMS, "path too long");
-    return CPB_OK;
-}
 cpb_status cpb_merkle_poseidon_verify_ragged_batch_dev(cpb_poseidon_ctx* leaf, cpb_poseidon_ctx* node, const uint64_t* root,
                                                        const uint64_t* values, const uint64_t* offsets, const uint64_t* leaf_sibling_hashes,
                                                        const uint64_t* auth_paths, size_t path_len, const uint64_t* leaf_indexes,
@@ -1143,23 +1091,14 @@ cpb_status cpb_merkle_poseidon_verify_ragged_batch(cpb_poseidon_ctx* leaf, cpb_p
     std::lock_guard<std::mutex> lk(leaf->mu);
     DeviceGuard g(leaf->device);
     cudaStream_t st = leaf->stream;
-    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t b_sib = n * 32, b_path = n * path_len * 32, b_idx = n * 8;
-    const size_t o_sib = 256, o_path = o_sib + up(b_sib), o_idx = o_path + up(b_path), front = o_idx + up(b_idx);
-    u64* d_off = nullptr;
-    u32* d_val = nullptr;
-    CPB_TRY(stage_ragged(leaf->s_in, front, values, offsets, n, st, d_off, d_val));    // the fixed-size arrays go in front
-    CPB_TRY(leaf->s_out.reserve(n));
-    char* d = (char*)leaf->s_in.ptr;
-    CPB_CUDA(cudaMemcpyAsync(d, root, 32, cudaMemcpyHostToDevice, st));
-    CPB_CUDA(cudaMemcpyAsync(d + o_sib, leaf_sibling_hashes, b_sib, cudaMemcpyHostToDevice, st));
-    if (b_path) CPB_CUDA(cudaMemcpyAsync(d + o_path, auth_paths, b_path, cudaMemcpyHostToDevice, st));
-    CPB_CUDA(cudaMemcpyAsync(d + o_idx, leaf_indexes, b_idx, cudaMemcpyHostToDevice, st));
-    CPB_TRY(launch_verify_ragged(leaf, node, (const u32*)d, d_val, offsets[0], d_off, (const u32*)(d + o_sib), (const u32*)(d + o_path),
-                                 (int)path_len, (const unsigned long long*)(d + o_idx), (uint8_t*)leaf->s_out.ptr, n, st));
-    CPB_CUDA(cudaMemcpyAsync(ok, leaf->s_out.ptr, n, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    HostStage S(leaf->arena, st);
+    const size_t o_root = S.in(root, 32), o_sib = S.in(leaf_sibling_hashes, n * 32), o_path = S.in(auth_paths, n * path_len * 32),
+                 o_idx = S.in(leaf_indexes, n * 8), o_off = S.in(offsets, (n + 1) * 8),
+                 o_val = S.in(values + 4 * offsets[0], (offsets[n] - offsets[0]) * 32), o_ok = S.out(ok, n);
+    CPB_TRY(S.upload());
+    CPB_TRY(launch_verify_ragged(leaf, node, S.at<u32>(o_root), S.at<u32>(o_val), offsets[0], S.at<u64>(o_off), S.at<u32>(o_sib),
+                                 S.at<u32>(o_path), (int)path_len, S.at<unsigned long long>(o_idx), S.at<uint8_t>(o_ok), n, st));
+    return S.download();
     });
 }
 
@@ -1194,7 +1133,7 @@ cpb_status launch_duplex(cpb_poseidon_ctx* c, u32* states, const DuplexOp& op, s
 }
 
 // One call on the whole batch.  `in_bytes` / `out_bytes`: the host form's copies of op.in or op.bytes and of op.out (host == true:
-// states and every buffer of op are host memory, staged through the context's scratch).  n == 0 or an absorb of nothing only
+// states and every buffer of op are host memory, staged through the context's arena).  n == 0 or an absorb of nothing only
 // advances the mode.
 cpb_status duplex_call(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* mode, DuplexOp op, size_t n, size_t in_bytes,
                        size_t out_bytes, bool host, cudaStream_t st) {
@@ -1208,21 +1147,15 @@ cpb_status duplex_call(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode* m
             CPB_TRY(launch_duplex(c, (u32*)states, op, n, st));
         } else {
             std::lock_guard<std::mutex> lk(c->mu);
-            const size_t s_b = n * (size_t)c->dev.t * 32;
-            CPB_TRY(c->s_aux.reserve(s_b));
-            CPB_TRY(c->s_in.reserve(in_bytes ? in_bytes : 32));
-            CPB_TRY(c->s_out.reserve(out_bytes ? out_bytes : 32));
-            CPB_CUDA(cudaMemcpyAsync(c->s_aux.ptr, states, s_b, cudaMemcpyHostToDevice, c->stream));
+            HostStage S(c->arena, c->stream);
             const void* src = op.kind == kAbsorbBytes ? (const void*)op.bytes : (const void*)op.in;
-            if (in_bytes) CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, src, in_bytes, cudaMemcpyHostToDevice, c->stream));
-            u32* host_out = op.out;
-            op.in = (const u32*)c->s_in.ptr;
-            op.bytes = (const unsigned char*)c->s_in.ptr;
-            op.out = (u32*)c->s_out.ptr;
-            CPB_TRY(launch_duplex(c, (u32*)c->s_aux.ptr, op, n, c->stream));
-            CPB_CUDA(cudaMemcpyAsync(states, c->s_aux.ptr, s_b, cudaMemcpyDeviceToHost, c->stream));
-            if (out_bytes) CPB_CUDA(cudaMemcpyAsync(host_out, c->s_out.ptr, out_bytes, cudaMemcpyDeviceToHost, c->stream));
-            CPB_CUDA(cudaStreamSynchronize(c->stream));
+            const size_t o_s = S.inout(states, n * (size_t)c->dev.t * 32), o_in = S.in(src, in_bytes), o_out = S.out(op.out, out_bytes);
+            CPB_TRY(S.upload());
+            op.in = S.at<u32>(o_in);
+            op.bytes = S.at<unsigned char>(o_in);
+            op.out = S.at<u32>(o_out);
+            CPB_TRY(launch_duplex(c, S.at<u32>(o_s), op, n, c->stream));
+            CPB_TRY(S.download());
         }
     }
     mode->squeezing = p.mode.squeezing;
@@ -1308,30 +1241,23 @@ cpb_status duplex_ragged(cpb_poseidon_ctx* c, uint64_t* states, cpb_sponge_mode*
     DeviceGuard g(c->device);
     if (!host) return duplex_ragged_dev(c, (u32*)states, R, (cudaStream_t)stream);
 
-    // host form: states in s_aux; the modes, the offsets and the data span in s_in; the output span in s_out
+    // host form: the states and the modes go up and come back; the data span goes up (absorb) or comes back (squeeze)
     std::lock_guard<std::mutex> lk(c->mu);
-    cudaStream_t st = c->stream;
+    HostStage S(c->arena, c->stream);
     const bool squeeze = kind >= kSqueeze;
-    const size_t s_b = n * (size_t)c->dev.t * 32, m_b = n * sizeof(cpb_sponge_mode), span = (size_t)(offsets[n] - offsets[0]);
-    CPB_TRY(c->s_aux.reserve(s_b));
-    u64* d_off = nullptr;
-    u32* d_val = nullptr;
-    CPB_TRY(stage_ragged(c->s_in, m_b, data, offsets, n, st, d_off, d_val, squeeze ? 0 : unit));
-    if (squeeze) CPB_TRY(c->s_out.reserve(span ? span * 32 : 32));
-    CPB_CUDA(cudaMemcpyAsync(c->s_aux.ptr, states, s_b, cudaMemcpyHostToDevice, st));
-    CPB_CUDA(cudaMemcpyAsync(c->s_in.ptr, modes, m_b, cudaMemcpyHostToDevice, st));
-    R.modes = (u64*)c->s_in.ptr;
-    R.offsets = d_off;
+    char* span = (char*)data + unit * offsets[0];
+    const size_t span_b = (size_t)(offsets[n] - offsets[0]) * unit;
+    const size_t o_s = S.inout(states, n * (size_t)c->dev.t * 32), o_m = S.inout(modes, n * sizeof(cpb_sponge_mode)),
+                 o_off = S.in(offsets, (n + 1) * 8), o_val = squeeze ? S.out(span, span_b) : S.in(span, span_b);
+    CPB_TRY(S.upload());
+    R.modes = S.at<u64>(o_m);
+    R.offsets = S.at<u64>(o_off);
     R.vbase = offsets[0];
-    R.in = d_val;
-    R.bytes = (const unsigned char*)d_val;
-    R.out = squeeze ? (u32*)c->s_out.ptr : nullptr;
-    CPB_TRY(duplex_ragged_dev(c, (u32*)c->s_aux.ptr, R, st));
-    CPB_CUDA(cudaMemcpyAsync(states, c->s_aux.ptr, s_b, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaMemcpyAsync(modes, c->s_in.ptr, m_b, cudaMemcpyDeviceToHost, st));
-    if (squeeze && span) CPB_CUDA(cudaMemcpyAsync((uint64_t*)data + 4 * offsets[0], c->s_out.ptr, span * 32, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaStreamSynchronize(st));
-    return CPB_OK;
+    R.in = S.at<u32>(o_val);
+    R.bytes = S.at<unsigned char>(o_val);
+    R.out = squeeze ? S.at<u32>(o_val) : nullptr;
+    CPB_TRY(duplex_ragged_dev(c, S.at<u32>(o_s), R, c->stream));
+    return S.download();
 }
 
 }  // namespace

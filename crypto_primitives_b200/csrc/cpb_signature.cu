@@ -279,6 +279,7 @@ struct cpb_te_base_ctx {
     u32* d_consts = nullptr;
     cudaStream_t stream = nullptr;
     std::mutex mu;
+    Scratch arena;      // the host-pointer entry points' device copies (HostStage), under mu
 };
 
 namespace {
@@ -395,45 +396,55 @@ template <class Fn> cpb_status on_curve(const cpb_te_base_ctx* c, Fn&& fn) {
     return fail(CPB_INTERNAL_ERROR, "context of curve %d", c->curve_id);
 }
 
-// Host-form plumbing: uploads on the context's stream, one synchronisation at the end.
-struct HostCall {
-    cudaStream_t st;
-    std::vector<void*> bufs;
-    explicit HostCall(cudaStream_t s) : st(s) {}
-    ~HostCall() {
-        for (void* p : bufs) cudaFreeAsync(p, st);
-        cudaStreamSynchronize(st);
+// The checks of each operation, in the header's order, shared by its two forms; n == 0 passes them and the call is done.  `host`: the
+// host form's checks of its host arrays, which come before the context.
+cpb_status check_msgs(const uint8_t* msgs, const uint64_t* off, size_t n) {
+    CPB_TRY(check_offsets(off, n));
+    if (!msgs && off[n] != off[0]) return fail(CPB_NULL_POINTER, "null messages");
+    return CPB_OK;
+}
+cpb_status check_plain(const cpb_te_base_ctx* c, bool buffers, size_t n) {       // base_mul, encrypt, decrypt
+    CPB_TRY(check_n(n));
+    if (n == 0) return CPB_OK;
+    if (!buffers) return fail(CPB_NULL_POINTER, "null array");
+    return ctx_check(c);
+}
+cpb_status check_signing(const cpb_te_base_ctx* c, bool buffers, const uint8_t* msgs, const uint64_t* off, size_t n, bool host) {
+    CPB_TRY(check_n(n));
+    if (n == 0) return CPB_OK;
+    if (!buffers) return fail(CPB_NULL_POINTER, "null array");
+    if (host) CPB_TRY(check_msgs(msgs, off, n));
+    return ctx_check(c);
+}
+cpb_status check_randomize(const cpb_te_base_ctx* c, bool buffers, size_t len, size_t stride, size_t n, bool public_key, bool host) {
+    CPB_TRY(check_n(n));
+    if (n == 0) return CPB_OK;
+    if (!buffers) return fail(CPB_NULL_POINTER, "null array");
+    if (host && len > stride && n > 1) return fail(CPB_BAD_LENGTH, "randomness length %zu exceeds the stride %zu", len, stride);
+    if (public_key) CPB_TRY(check_rand_len(len));
+    return ctx_check(c);
+}
+cpb_status check_blake2s(const uint8_t* in, const uint64_t* offsets, bool buffers, size_t n, bool host) {
+    CPB_TRY(check_n(n));
+    if (n == 0) return CPB_OK;
+    if (!buffers) return fail(CPB_NULL_POINTER, "null array");
+    if (host) {
+        CPB_TRY(check_offsets(offsets, n));
+        if (!in && offsets[n] != offsets[0]) return fail(CPB_NULL_POINTER, "null input");
     }
-    template <class T> cpb_status alloc(T*& d, size_t bytes) {
-        void* p = nullptr;
-        CPB_CUDA(cudaMallocAsync(&p, bytes ? bytes : 1, st));
-        bufs.push_back(p);
-        d = (T*)p;
-        return CPB_OK;
-    }
-    template <class T> cpb_status up(T*& d, const void* h, size_t bytes) {
-        CPB_TRY(alloc(d, bytes));
-        if (bytes) CPB_CUDA(cudaMemcpyAsync((void*)d, h, bytes, cudaMemcpyHostToDevice, st));
-        return CPB_OK;
-    }
-    cpb_status down(void* h, const void* d, size_t bytes) {
-        if (bytes) CPB_CUDA(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st));
-        CPB_CUDA(cudaStreamSynchronize(st));
-        return CPB_OK;
-    }
-    // ragged messages: only bytes [off[0], off[n]) are copied; device offsets are rebased to start at 0
-    cpb_status messages(const uint8_t*& d_msgs, const u64*& d_off, const uint8_t* msgs, const uint64_t* off, size_t n) {
-        std::vector<uint64_t> rel(n + 1);
-        for (size_t i = 0; i <= n; i++) rel[i] = off[i] - off[0];
-        uint8_t* m = nullptr;
-        u64* o = nullptr;
-        CPB_TRY(up(m, msgs + off[0], rel[n]));
-        CPB_TRY(up(o, rel.data(), 8 * (n + 1)));
-        d_msgs = m;
-        d_off = o;
-        return CPB_OK;
-    }
-};
+    return CPB_OK;
+}
+cpb_status blake2s_dev(const uint8_t* in, const u64* offsets, const uint8_t* randomness32, uint8_t* out32, size_t n, cudaStream_t st) {
+    k_blake2s_commit<<<grid_of(n), kSigBlock, 0, st>>>(in, offsets, randomness32, out32, (long)n);
+    return launched("k_blake2s_commit");
+}
+
+// Ragged messages go up as the span [off[0], off[n]) with offsets rebased to start at 0.
+std::vector<uint64_t> rebased(const uint64_t* off, size_t n) {
+    std::vector<uint64_t> rel(n + 1);
+    for (size_t i = 0; i <= n; i++) rel[i] = off[i] - off[0];
+    return rel;
+}
 
 // Affine doubling over the host field (a = -1, either curve): x3 = 2xy / (1 + d x^2 y^2), y3 = (y^2 + x^2) / (1 - d x^2 y^2).
 void host_double(const host::Field& F, const host::Fe& d, host::Fe& x, host::Fe& y) {
@@ -525,10 +536,8 @@ void cpb_te_base_ctx_destroy(cpb_te_base_ctx* c) {
 // ---- device-pointer forms
 cpb_status cpb_te_base_mul_batch_dev(cpb_te_base_ctx* c, const uint64_t* scalars, uint64_t* out_xy, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_plain(c, scalars && out_xy, n));
     if (n == 0) return CPB_OK;
-    if (!scalars || !out_xy) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
     return on_curve(c, [&](auto k) { return base_mul_dev<decltype(k)>(c, (const u32*)scalars, 8, (u32*)out_xy, n, (cudaStream_t)stream); });
     });
@@ -537,10 +546,8 @@ cpb_status cpb_te_base_mul_batch_dev(cpb_te_base_ctx* c, const uint64_t* scalars
 cpb_status cpb_schnorr_sign_batch_dev(cpb_te_base_ctx* c, const uint8_t* salt, const uint64_t* sks, const uint64_t* nonces, const uint8_t* msgs,
                                       const uint64_t* msg_offsets, uint64_t* sigs_out, uint8_t* signed_out, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_signing(c, salt && sks && nonces && msg_offsets && sigs_out && signed_out, msgs, msg_offsets, n, false));
     if (n == 0) return CPB_OK;
-    if (!salt || !sks || !nonces || !msg_offsets || !sigs_out || !signed_out) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
     return on_curve(c, [&](auto k) {
         return sign_dev<decltype(k)>(c, salt_of(salt), (const u32*)sks, (const u32*)nonces, msgs, (const u64*)msg_offsets, (u32*)sigs_out,
@@ -552,10 +559,8 @@ cpb_status cpb_schnorr_sign_batch_dev(cpb_te_base_ctx* c, const uint8_t* salt, c
 cpb_status cpb_schnorr_verify_batch_dev(cpb_te_base_ctx* c, const uint8_t* salt, const uint64_t* pks_xy, const uint8_t* msgs,
                                         const uint64_t* msg_offsets, const uint64_t* sigs, uint8_t* ok_out, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_signing(c, salt && pks_xy && msg_offsets && sigs && ok_out, msgs, msg_offsets, n, false));
     if (n == 0) return CPB_OK;
-    if (!salt || !pks_xy || !msg_offsets || !sigs || !ok_out) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
     return on_curve(c, [&](auto k) {
         return verify_dev<decltype(k)>(c, salt_of(salt), (const u32*)pks_xy, msgs, (const u64*)msg_offsets, (const u32*)sigs, ok_out, n,
@@ -567,11 +572,8 @@ cpb_status cpb_schnorr_verify_batch_dev(cpb_te_base_ctx* c, const uint8_t* salt,
 cpb_status cpb_schnorr_randomize_public_key_batch_dev(cpb_te_base_ctx* c, const uint64_t* pks_xy, const uint8_t* randomness, size_t len,
                                                       size_t stride, uint64_t* out_xy, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_randomize(c, pks_xy && out_xy && (!len || randomness), len, stride, n, true, false));
     if (n == 0) return CPB_OK;
-    if (!pks_xy || !out_xy || (len && !randomness)) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(check_rand_len(len));
-    CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
     return on_curve(c, [&](auto k) {
         return rand_pk_dev<decltype(k)>(c, (const u32*)pks_xy, randomness, len, stride, (u32*)out_xy, n, (cudaStream_t)stream);
@@ -582,10 +584,8 @@ cpb_status cpb_schnorr_randomize_public_key_batch_dev(cpb_te_base_ctx* c, const 
 cpb_status cpb_schnorr_randomize_signature_batch_dev(cpb_te_base_ctx* c, const uint64_t* sigs, const uint8_t* randomness, size_t len,
                                                      size_t stride, uint64_t* sigs_out, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_randomize(c, sigs && sigs_out && (!len || randomness), len, stride, n, false, false));
     if (n == 0) return CPB_OK;
-    if (!sigs || !sigs_out || (len && !randomness)) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
     return on_curve(c, [&](auto k) {
         return rand_sig_dev<decltype(k)>(c, (const u32*)sigs, randomness, len, stride, (u32*)sigs_out, n, (cudaStream_t)stream);
@@ -596,10 +596,8 @@ cpb_status cpb_schnorr_randomize_signature_batch_dev(cpb_te_base_ctx* c, const u
 cpb_status cpb_elgamal_encrypt_batch_dev(cpb_te_base_ctx* c, const uint64_t* pks_xy, const uint64_t* msgs_xy, const uint64_t* rands,
                                          uint64_t* ciphertexts_out, size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_plain(c, pks_xy && msgs_xy && rands && ciphertexts_out, n));
     if (n == 0) return CPB_OK;
-    if (!pks_xy || !msgs_xy || !rands || !ciphertexts_out) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
     return on_curve(c, [&](auto k) {
         return encrypt_dev<decltype(k)>(c, (const u32*)pks_xy, (const u32*)msgs_xy, (const u32*)rands, (u32*)ciphertexts_out, n, (cudaStream_t)stream);
@@ -610,10 +608,8 @@ cpb_status cpb_elgamal_encrypt_batch_dev(cpb_te_base_ctx* c, const uint64_t* pks
 cpb_status cpb_elgamal_decrypt_batch_dev(cpb_te_base_ctx* c, const uint64_t* sks, const uint64_t* ciphertexts, uint64_t* msgs_out, size_t n,
                                          void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_plain(c, sks && ciphertexts && msgs_out, n));
     if (n == 0) return CPB_OK;
-    if (!sks || !ciphertexts || !msgs_out) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     DeviceGuard g(c->device);
     return on_curve(c, [&](auto k) {
         return decrypt_dev<decltype(k)>(c, (const u32*)sks, (const u32*)ciphertexts, (u32*)msgs_out, n, (cudaStream_t)stream);
@@ -624,195 +620,156 @@ cpb_status cpb_elgamal_decrypt_batch_dev(cpb_te_base_ctx* c, const uint64_t* sks
 cpb_status cpb_blake2s_commit_batch_dev(int device, const uint8_t* in, const uint64_t* offsets, const uint8_t* randomness32, uint8_t* out32,
                                         size_t n, void* stream) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_blake2s(in, offsets, offsets && randomness32 && out32, n, false));
     if (n == 0) return CPB_OK;
-    if (!offsets || !randomness32 || !out32) return fail(CPB_NULL_POINTER, "null array");
     DeviceGuard g(device);
     if (!g.ok) { cudaGetLastError(); return fail(CPB_NO_DEVICE, "cudaSetDevice(%d) failed: no usable CUDA device", device); }
     CPB_TRY(check_device_arch(device));
-    k_blake2s_commit<<<grid_of(n), kSigBlock, 0, (cudaStream_t)stream>>>(in, (const u64*)offsets, randomness32, out32, (long)n);
-    return launched("k_blake2s_commit");
+    return blake2s_dev(in, (const u64*)offsets, randomness32, out32, n, (cudaStream_t)stream);
     });
 }
 
-// ---- host-pointer forms
+// ---- host-pointer forms: the _dev form's core on the context arena and stream (HostStage), under the context mutex
 cpb_status cpb_te_base_mul_batch(cpb_te_base_ctx* c, const uint64_t* scalars, uint64_t* out_xy, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_plain(c, scalars && out_xy, n));
     if (n == 0) return CPB_OK;
-    if (!scalars || !out_xy) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    HostCall h(c->stream);
-    u32 *d_s, *d_o;
-    CPB_TRY(h.up(d_s, scalars, 32 * n));
-    CPB_TRY(h.alloc(d_o, 64 * n));
-    CPB_TRY(on_curve(c, [&](auto k) { return base_mul_dev<decltype(k)>(c, d_s, 8, d_o, n, c->stream); }));
-    return h.down(out_xy, d_o, 64 * n);
+    HostStage S(c->arena, c->stream);
+    const size_t o_s = S.in(scalars, 32 * n), o_o = S.out(out_xy, 64 * n);
+    CPB_TRY(S.upload());
+    CPB_TRY(on_curve(c, [&](auto k) { return base_mul_dev<decltype(k)>(c, S.at<u32>(o_s), 8, S.at<u32>(o_o), n, c->stream); }));
+    return S.download();
     });
 }
 
 cpb_status cpb_schnorr_sign_batch(cpb_te_base_ctx* c, const uint8_t* salt, const uint64_t* sks, const uint64_t* nonces, const uint8_t* msgs,
                                   const uint64_t* msg_offsets, uint64_t* sigs_out, uint8_t* signed_out, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_signing(c, salt && sks && nonces && msg_offsets && sigs_out && signed_out, msgs, msg_offsets, n, true));
     if (n == 0) return CPB_OK;
-    if (!salt || !sks || !nonces || !msg_offsets || !sigs_out || !signed_out) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(check_offsets(msg_offsets, n));
-    if (!msgs && msg_offsets[n] != msg_offsets[0]) return fail(CPB_NULL_POINTER, "null messages");
-    CPB_TRY(ctx_check(c));
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    HostCall h(c->stream);
-    u32 *d_sk, *d_k, *d_sig;
-    uint8_t* d_ok;
-    const uint8_t* d_m;
-    const u64* d_off;
-    CPB_TRY(h.up(d_sk, sks, 32 * n));
-    CPB_TRY(h.up(d_k, nonces, 32 * n));
-    CPB_TRY(h.messages(d_m, d_off, msgs, msg_offsets, n));
-    CPB_TRY(h.alloc(d_sig, 64 * n));
-    CPB_TRY(h.alloc(d_ok, n));
-    CPB_TRY(on_curve(c, [&](auto k) { return sign_dev<decltype(k)>(c, salt_of(salt), d_sk, d_k, d_m, d_off, d_sig, d_ok, n, c->stream); }));
-    CPB_CUDA(cudaMemcpyAsync(signed_out, d_ok, n, cudaMemcpyDeviceToHost, c->stream));
-    return h.down(sigs_out, d_sig, 64 * n);
+    const std::vector<uint64_t> rel = rebased(msg_offsets, n);
+    HostStage S(c->arena, c->stream);
+    const size_t o_sk = S.in(sks, 32 * n), o_k = S.in(nonces, 32 * n), o_m = S.in(msgs + msg_offsets[0], rel[n]),
+                 o_off = S.in(rel.data(), 8 * (n + 1)), o_sig = S.out(sigs_out, 64 * n), o_ok = S.out(signed_out, n);
+    CPB_TRY(S.upload());
+    CPB_TRY(on_curve(c, [&](auto k) {
+        return sign_dev<decltype(k)>(c, salt_of(salt), S.at<u32>(o_sk), S.at<u32>(o_k), S.at<uint8_t>(o_m), S.at<u64>(o_off), S.at<u32>(o_sig),
+                                     S.at<uint8_t>(o_ok), n, c->stream);
+    }));
+    return S.download();
     });
 }
 
 cpb_status cpb_schnorr_verify_batch(cpb_te_base_ctx* c, const uint8_t* salt, const uint64_t* pks_xy, const uint8_t* msgs,
                                     const uint64_t* msg_offsets, const uint64_t* sigs, uint8_t* ok_out, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_signing(c, salt && pks_xy && msg_offsets && sigs && ok_out, msgs, msg_offsets, n, true));
     if (n == 0) return CPB_OK;
-    if (!salt || !pks_xy || !msg_offsets || !sigs || !ok_out) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(check_offsets(msg_offsets, n));
-    if (!msgs && msg_offsets[n] != msg_offsets[0]) return fail(CPB_NULL_POINTER, "null messages");
-    CPB_TRY(ctx_check(c));
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    HostCall h(c->stream);
-    u32 *d_pk, *d_sig;
-    uint8_t* d_ok;
-    const uint8_t* d_m;
-    const u64* d_off;
-    CPB_TRY(h.up(d_pk, pks_xy, 64 * n));
-    CPB_TRY(h.up(d_sig, sigs, 64 * n));
-    CPB_TRY(h.messages(d_m, d_off, msgs, msg_offsets, n));
-    CPB_TRY(h.alloc(d_ok, n));
-    CPB_TRY(on_curve(c, [&](auto k) { return verify_dev<decltype(k)>(c, salt_of(salt), d_pk, d_m, d_off, d_sig, d_ok, n, c->stream); }));
-    return h.down(ok_out, d_ok, n);
+    const std::vector<uint64_t> rel = rebased(msg_offsets, n);
+    HostStage S(c->arena, c->stream);
+    const size_t o_pk = S.in(pks_xy, 64 * n), o_sig = S.in(sigs, 64 * n), o_m = S.in(msgs + msg_offsets[0], rel[n]),
+                 o_off = S.in(rel.data(), 8 * (n + 1)), o_ok = S.out(ok_out, n);
+    CPB_TRY(S.upload());
+    CPB_TRY(on_curve(c, [&](auto k) {
+        return verify_dev<decltype(k)>(c, salt_of(salt), S.at<u32>(o_pk), S.at<uint8_t>(o_m), S.at<u64>(o_off), S.at<u32>(o_sig),
+                                       S.at<uint8_t>(o_ok), n, c->stream);
+    }));
+    return S.download();
     });
 }
 
 cpb_status cpb_schnorr_randomize_public_key_batch(cpb_te_base_ctx* c, const uint64_t* pks_xy, const uint8_t* randomness, size_t len,
                                                   size_t stride, uint64_t* out_xy, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_randomize(c, pks_xy && out_xy && (!len || randomness), len, stride, n, true, true));
     if (n == 0) return CPB_OK;
-    if (!pks_xy || !out_xy || (len && !randomness)) return fail(CPB_NULL_POINTER, "null array");
-    if (len > stride && n > 1) return fail(CPB_BAD_LENGTH, "randomness length %zu exceeds the stride %zu", len, stride);
-    CPB_TRY(check_rand_len(len));
-    CPB_TRY(ctx_check(c));
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    HostCall h(c->stream);
-    u32 *d_pk, *d_o;
-    uint8_t* d_r;
-    const size_t rbytes = n ? (n - 1) * stride + len : 0;
-    CPB_TRY(h.up(d_pk, pks_xy, 64 * n));
-    CPB_TRY(h.up(d_r, randomness, rbytes));
-    CPB_TRY(h.alloc(d_o, 64 * n));
-    CPB_TRY(cpb_schnorr_randomize_public_key_batch_dev(c, (const uint64_t*)d_pk, d_r, len, stride, (uint64_t*)d_o, n, c->stream));
-    return h.down(out_xy, d_o, 64 * n);
+    HostStage S(c->arena, c->stream);
+    const size_t o_pk = S.in(pks_xy, 64 * n), o_r = S.in(randomness, (n - 1) * stride + len), o_o = S.out(out_xy, 64 * n);
+    CPB_TRY(S.upload());
+    CPB_TRY(on_curve(c, [&](auto k) {
+        return rand_pk_dev<decltype(k)>(c, S.at<u32>(o_pk), S.at<uint8_t>(o_r), len, stride, S.at<u32>(o_o), n, c->stream);
+    }));
+    return S.download();
     });
 }
 
 cpb_status cpb_schnorr_randomize_signature_batch(cpb_te_base_ctx* c, const uint64_t* sigs, const uint8_t* randomness, size_t len, size_t stride,
                                                  uint64_t* sigs_out, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_randomize(c, sigs && sigs_out && (!len || randomness), len, stride, n, false, true));
     if (n == 0) return CPB_OK;
-    if (!sigs || !sigs_out || (len && !randomness)) return fail(CPB_NULL_POINTER, "null array");
-    if (len > stride && n > 1) return fail(CPB_BAD_LENGTH, "randomness length %zu exceeds the stride %zu", len, stride);
-    CPB_TRY(ctx_check(c));
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    HostCall h(c->stream);
-    u32 *d_s, *d_o;
-    uint8_t* d_r;
-    const size_t rbytes = n ? (n - 1) * stride + len : 0;
-    CPB_TRY(h.up(d_s, sigs, 64 * n));
-    CPB_TRY(h.up(d_r, randomness, rbytes));
-    CPB_TRY(h.alloc(d_o, 64 * n));
-    CPB_TRY(cpb_schnorr_randomize_signature_batch_dev(c, (const uint64_t*)d_s, d_r, len, stride, (uint64_t*)d_o, n, c->stream));
-    return h.down(sigs_out, d_o, 64 * n);
+    HostStage S(c->arena, c->stream);
+    const size_t o_s = S.in(sigs, 64 * n), o_r = S.in(randomness, (n - 1) * stride + len), o_o = S.out(sigs_out, 64 * n);
+    CPB_TRY(S.upload());
+    CPB_TRY(on_curve(c, [&](auto k) {
+        return rand_sig_dev<decltype(k)>(c, S.at<u32>(o_s), S.at<uint8_t>(o_r), len, stride, S.at<u32>(o_o), n, c->stream);
+    }));
+    return S.download();
     });
 }
 
 cpb_status cpb_elgamal_encrypt_batch(cpb_te_base_ctx* c, const uint64_t* pks_xy, const uint64_t* msgs_xy, const uint64_t* rands,
                                      uint64_t* ciphertexts_out, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_plain(c, pks_xy && msgs_xy && rands && ciphertexts_out, n));
     if (n == 0) return CPB_OK;
-    if (!pks_xy || !msgs_xy || !rands || !ciphertexts_out) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    HostCall h(c->stream);
-    u32 *d_pk, *d_m, *d_r, *d_o;
-    CPB_TRY(h.up(d_pk, pks_xy, 64 * n));
-    CPB_TRY(h.up(d_m, msgs_xy, 64 * n));
-    CPB_TRY(h.up(d_r, rands, 32 * n));
-    CPB_TRY(h.alloc(d_o, 128 * n));
-    CPB_TRY(on_curve(c, [&](auto k) { return encrypt_dev<decltype(k)>(c, d_pk, d_m, d_r, d_o, n, c->stream); }));
-    return h.down(ciphertexts_out, d_o, 128 * n);
+    HostStage S(c->arena, c->stream);
+    const size_t o_pk = S.in(pks_xy, 64 * n), o_m = S.in(msgs_xy, 64 * n), o_r = S.in(rands, 32 * n), o_o = S.out(ciphertexts_out, 128 * n);
+    CPB_TRY(S.upload());
+    CPB_TRY(on_curve(c, [&](auto k) {
+        return encrypt_dev<decltype(k)>(c, S.at<u32>(o_pk), S.at<u32>(o_m), S.at<u32>(o_r), S.at<u32>(o_o), n, c->stream);
+    }));
+    return S.download();
     });
 }
 
 cpb_status cpb_elgamal_decrypt_batch(cpb_te_base_ctx* c, const uint64_t* sks, const uint64_t* ciphertexts, uint64_t* msgs_out, size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_plain(c, sks && ciphertexts && msgs_out, n));
     if (n == 0) return CPB_OK;
-    if (!sks || !ciphertexts || !msgs_out) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(ctx_check(c));
     std::lock_guard<std::mutex> lk(c->mu);
     DeviceGuard g(c->device);
-    HostCall h(c->stream);
-    u32 *d_sk, *d_ct, *d_o;
-    CPB_TRY(h.up(d_sk, sks, 32 * n));
-    CPB_TRY(h.up(d_ct, ciphertexts, 128 * n));
-    CPB_TRY(h.alloc(d_o, 64 * n));
-    CPB_TRY(cpb_elgamal_decrypt_batch_dev(c, (const uint64_t*)d_sk, (const uint64_t*)d_ct, (uint64_t*)d_o, n, c->stream));
-    return h.down(msgs_out, d_o, 64 * n);
+    HostStage S(c->arena, c->stream);
+    const size_t o_sk = S.in(sks, 32 * n), o_ct = S.in(ciphertexts, 128 * n), o_o = S.out(msgs_out, 64 * n);
+    CPB_TRY(S.upload());
+    CPB_TRY(on_curve(c, [&](auto k) { return decrypt_dev<decltype(k)>(c, S.at<u32>(o_sk), S.at<u32>(o_ct), S.at<u32>(o_o), n, c->stream); }));
+    return S.download();
     });
 }
 
+// No context: a local arena and a stream of its own, both released before the call returns.
 cpb_status cpb_blake2s_commit_batch(int device, const uint8_t* in, const uint64_t* offsets, const uint8_t* randomness32, uint8_t* out32,
                                     size_t n) {
     return cpb::guarded([&]() -> cpb_status {
-    CPB_TRY(check_n(n));
+    CPB_TRY(check_blake2s(in, offsets, offsets && randomness32 && out32, n, true));
     if (n == 0) return CPB_OK;
-    if (!offsets || !randomness32 || !out32) return fail(CPB_NULL_POINTER, "null array");
-    CPB_TRY(check_offsets(offsets, n));
-    if (!in && offsets[n] != offsets[0]) return fail(CPB_NULL_POINTER, "null input");
     DeviceGuard g(device);
     if (!g.ok) { cudaGetLastError(); return fail(CPB_NO_DEVICE, "cudaSetDevice(%d) failed: no usable CUDA device", device); }
     CPB_TRY(check_device_arch(device));
     cudaStream_t st = nullptr;
     CPB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    cpb_status r;
-    {
-        HostCall h(st);
-        const uint8_t* d_in;
-        const u64* d_off;
-        uint8_t *d_r, *d_o;
-        r = h.messages(d_in, d_off, in, offsets, n);
-        if (r == CPB_OK) r = h.up(d_r, randomness32, 32 * n);
-        if (r == CPB_OK) r = h.alloc(d_o, 32 * n);
-        if (r == CPB_OK) r = cpb_blake2s_commit_batch_dev(device, d_in, (const uint64_t*)d_off, d_r, d_o, n, st);
-        if (r == CPB_OK) r = h.down(out32, d_o, 32 * n);
-    }
+    Scratch arena;
+    const std::vector<uint64_t> rel = rebased(offsets, n);
+    const cpb_status r = [&]() -> cpb_status {
+        HostStage S(arena, st);
+        const size_t o_in = S.in(in + offsets[0], rel[n]), o_off = S.in(rel.data(), 8 * (n + 1)), o_r = S.in(randomness32, 32 * n),
+                     o_o = S.out(out32, 32 * n);
+        CPB_TRY(S.upload());
+        CPB_TRY(blake2s_dev(S.at<uint8_t>(o_in), S.at<u64>(o_off), S.at<uint8_t>(o_r), S.at<uint8_t>(o_o), n, st));
+        return S.download();
+    }();
     cudaStreamDestroy(st);
     return r;
     });

@@ -123,8 +123,6 @@ struct UpdBuffers {
     void* extra() const { return b + o_extra; }
 };
 
-inline size_t upd_up(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // Plan offsets of an n-leaf tree and k updates (k > 0) into X; the buffer sizes into B.
 inline cpb_status upd_layout(UpdPlan& X, size_t n, size_t k, size_t extra, int W, cudaStream_t st, UpdBuffers& B) {
     X.h = log2_exact(n);
@@ -137,16 +135,16 @@ inline cpb_status upd_layout(UpdPlan& X, size_t n, size_t k, size_t extra, int W
     CPB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const unsigned*)nullptr, (unsigned*)nullptr, uk, st));
     B.tmp_b = sort_b > scan_b ? sort_b : scan_b;
     size_t o = 0;
-    B.o_kin = o; o += upd_up(8 * k);
-    B.o_kout = o; o += upd_up(8 * k);
-    B.o_pin = o; o += upd_up(4 * k);
-    B.o_pout = o; o += upd_up(4 * k);
-    B.o_flag = o; o += upd_up(4 * k);
-    B.o_scan = o; o += upd_up(4 * k);
-    B.o_U = o; o += upd_up(8 * k);
+    B.o_kin = o; o += align256(8 * k);
+    B.o_kout = o; o += align256(8 * k);
+    B.o_pin = o; o += align256(4 * k);
+    B.o_pout = o; o += align256(4 * k);
+    B.o_flag = o; o += align256(4 * k);
+    B.o_scan = o; o += align256(4 * k);
+    B.o_U = o; o += align256(8 * k);
     B.o_m = o; o += 256;
-    B.o_tmp = o; o += upd_up(B.tmp_b);
-    B.o_extra = o; o += upd_up(extra);
+    B.o_tmp = o; o += align256(B.tmp_b);
+    B.o_extra = o; o += align256(extra);
     B.o_scr = o; o += 4 * (size_t)W * (size_t)X.off[X.h + 1];
     B.total = o;
     return CPB_OK;
@@ -183,8 +181,8 @@ cpb_status upd_run_plan(const UpdBuffers& B, UpdPlan& X, const u64* idx, size_t 
 }
 
 // Host arrays (leaf_nodes: n elements, non_leaf_nodes: n - 1, W words each; arguments already checked, k > 0): only the siblings
-// the touched nodes read go up, only the touched nodes come back.  The device mirror of the tree (node->s_aux, 2n - 1 elements:
-// leaves, then inner nodes) is allocated but never filled beyond those siblings.  `in` (in_bytes) is uploaded as it is;
+// the touched nodes read go up, only the touched nodes come back.  The device mirror of the tree (2n - 1 elements in the node context's
+// arena: leaves, then inner nodes) is allocated but never filled beyond those siblings.  `in` (in_bytes) is uploaded as it is;
 // run(mirror_leaves, mirror_nodes, d_idx, d_in, d_root or NULL, d_applied, stream) is the _dev form on the mirror.
 template <int W, class Ctx, class Run>
 cpb_status upd_host_form(Ctx* node, uint64_t* leaf_nodes, uint64_t* non_leaf_nodes, size_t n, const uint64_t* indexes, const void* in,
@@ -199,43 +197,27 @@ cpb_status upd_host_form(Ctx* node, uint64_t* leaf_nodes, uint64_t* non_leaf_nod
     std::vector<uint64_t> read_vals((W / 2) * reads.size());
     for (size_t i = 0; i < reads.size(); i++) memcpy(&read_vals[(W / 2) * i], host_elem(reads[i]), EB);
 
+    const size_t nr = reads.size(), nw = writes.size();
+    std::vector<uint64_t> write_vals((W / 2) * nw);
+    unsigned char ok = 0;
     std::lock_guard<std::mutex> lk(node->mu);
     DeviceGuard g(node->device);
     cudaStream_t st = node->stream;
-    const size_t nr = reads.size(), nw = writes.size();
-    size_t o = 0;
-    const size_t o_idx = o; o += upd_up(8 * k);
-    const size_t o_in = o; o += upd_up(in_bytes ? in_bytes : 32);
-    const size_t o_root = o; o += upd_up(EB);
-    const size_t o_rpos = o; o += upd_up(8 * nr + 8);
-    const size_t o_rval = o; o += upd_up(EB * nr + EB);
-    const size_t o_wpos = o; o += upd_up(8 * nw);
-    CPB_TRY(node->s_in.reserve(o));
-    CPB_TRY(node->s_out.reserve(EB * nw + 256));
-    CPB_TRY(node->s_aux.reserve(EB * (2 * n - 1)));
-    char* d = (char*)node->s_in.ptr;
-    u32* mirror = (u32*)node->s_aux.ptr;
-    u32* d_out = (u32*)node->s_out.ptr;
-    unsigned char* d_applied = (unsigned char*)node->s_out.ptr + EB * nw;
-    CPB_CUDA(cudaMemcpyAsync(d + o_idx, indexes, 8 * k, cudaMemcpyHostToDevice, st));
-    if (in_bytes) CPB_CUDA(cudaMemcpyAsync(d + o_in, in, in_bytes, cudaMemcpyHostToDevice, st));
-    if (asserted_root) CPB_CUDA(cudaMemcpyAsync(d + o_root, asserted_root, EB, cudaMemcpyHostToDevice, st));
+    HostStage S(node->arena, st);
+    const size_t o_idx = S.in(indexes, 8 * k), o_in = S.in(in, in_bytes), o_root = S.in(asserted_root, asserted_root ? EB : 0),
+                 o_rpos = S.in(reads.data(), 8 * nr), o_rval = S.in(read_vals.data(), EB * nr), o_wpos = S.in(writes.data(), 8 * nw),
+                 o_out = S.out(write_vals.data(), EB * nw), o_applied = S.out(&ok, 1), o_mirror = S.dev(EB * (2 * n - 1));
+    CPB_TRY(S.upload());
+    u32* mirror = S.at<u32>(o_mirror);
     if (nr) {
-        CPB_CUDA(cudaMemcpyAsync(d + o_rpos, reads.data(), 8 * nr, cudaMemcpyHostToDevice, st));
-        CPB_CUDA(cudaMemcpyAsync(d + o_rval, read_vals.data(), EB * nr, cudaMemcpyHostToDevice, st));
-        k_upd_move<W><<<upd_grid(nr, kUpdBlock), kUpdBlock, 0, st>>>((const u32*)(d + o_rval), mirror, (const u64*)(d + o_rpos), nr, 0);
+        k_upd_move<W><<<upd_grid(nr, kUpdBlock), kUpdBlock, 0, st>>>(S.at<const u32>(o_rval), mirror, S.at<const u64>(o_rpos), nr, 0);
         CPB_CUDA(cudaGetLastError());
     }
-    CPB_CUDA(cudaMemcpyAsync(d + o_wpos, writes.data(), 8 * nw, cudaMemcpyHostToDevice, st));
-    CPB_TRY(run((uint64_t*)mirror, (uint64_t*)(mirror + W * n), (const uint64_t*)(d + o_idx), (const void*)(d + o_in),
-                asserted_root ? (const uint64_t*)(d + o_root) : nullptr, d_applied, st));
-    k_upd_move<W><<<upd_grid(nw, kUpdBlock), kUpdBlock, 0, st>>>(mirror, d_out, (const u64*)(d + o_wpos), nw, 1);
+    CPB_TRY(run((uint64_t*)mirror, (uint64_t*)(mirror + W * n), S.at<const uint64_t>(o_idx), S.at<const void>(o_in),
+                asserted_root ? S.at<const uint64_t>(o_root) : nullptr, S.at<unsigned char>(o_applied), st));
+    k_upd_move<W><<<upd_grid(nw, kUpdBlock), kUpdBlock, 0, st>>>(mirror, S.at<u32>(o_out), S.at<const u64>(o_wpos), nw, 1);
     CPB_CUDA(cudaGetLastError());
-    std::vector<uint64_t> write_vals((W / 2) * nw);
-    unsigned char ok = 0;
-    CPB_CUDA(cudaMemcpyAsync(write_vals.data(), d_out, EB * nw, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaMemcpyAsync(&ok, d_applied, 1, cudaMemcpyDeviceToHost, st));
-    CPB_CUDA(cudaStreamSynchronize(st));
+    CPB_TRY(S.download());
     if (ok)
         for (size_t i = 0; i < nw; i++) memcpy(host_elem(writes[i]), &write_vals[(W / 2) * i], EB);
     if (applied) *applied = ok;

@@ -26,7 +26,7 @@ struct cpb_pedersen_ctx {
     cpb::u32* d_table = nullptr;
     cudaStream_t stream = nullptr;
     std::mutex mu;
-    cpb::Scratch s_in, s_out, s_aux, s_rand;
+    cpb::Scratch arena;      // the host-pointer entry points' device copies (HostStage), under mu
 };
 
 namespace cpb {

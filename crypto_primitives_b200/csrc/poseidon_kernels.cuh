@@ -135,7 +135,7 @@ struct cpb_poseidon_ctx {
     const u32* d_tc_consts = nullptr;
     cudaStream_t stream = nullptr;
     std::mutex mu;
-    cpb::Scratch s_in, s_out, s_aux;
+    cpb::Scratch arena;                 // the host-pointer entry points' device copies (HostStage), under mu
     std::mutex side_mu;                 // guards creation of side[] only (mu may already be held by a host-pointer call)
     cudaStream_t side[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // subtree streams of the Merkle build
 };
